@@ -16,7 +16,12 @@
 //                   fill implements padding, elementStrides implement stride
 //   mode 2  WGRAD   C[Co,(tap,ci)] += sum_pix dY[pix,Co] * X[n,h+dh,w+dw,ci]   both MN-major, split-K.  bf16:
 //                   wgmma reads the MN-major tiles directly (transpose bits); tf32 (wgmma takes K-major tf32 only):
-//                   the consumers transpose each ring stage into a K-major shared buffer first
+//                   the consumers transpose each ring stage into a second, K-major ring while the wgmma of the
+//                   previous stage run
+//
+// The tile width BN is a template parameter, so each compiled mainloop issues one wgmma shape (4 per k-block, one
+// commit group).  The column pieces of a tail tile (PN columns) run a second, separately instantiated mainloop and
+// epilogue of the same kernel, chosen once per work unit.
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -30,11 +35,13 @@ constexpr int kMaxTaps = 16;
 constexpr int kStageABytes = 128 * 128;  // 128 rows x 128 B
 constexpr int kStatsBytes = 8 * 2 * 256 * 4;   // per-warp column sums / sums of squares (fused BatchNorm statistics)
 constexpr int kThreads = 384;            // producer warpgroup + 2 consumer warpgroups
+constexpr int kMmasPerKb = 4;            // a k-block is 128 B of K per row: 4 x k8 (tf32) / k16 (bf16) wgmma
+constexpr int kXStages = 2;              // tf32 WGRAD: stages of the K-major ring the consumers transpose into
 
 struct GemmParams {
   int mode, dtype;
   int M, N;               // logical output extent (rows, cols)
-  int block_n;            // 64 / 128 / 256
+  int block_n;            // 64 / 128 / 256 (the kernel's BN)
   int num_kb;             // k-blocks per tile
   int stages;
   int tiles_m, tiles_n, splits;
@@ -54,7 +61,6 @@ struct GemmParams {
   uint32_t a_lbo, a_sbo, b_lbo, b_sbo;
   uint32_t a_kadv, b_kadv;              // per wgmma k-step
   uint32_t a_half;                      // offset of the second consumer's 64 rows of A
-  int mmas_per_kb;
   int a_boxes, b_boxes;                 // TMA boxes per stage
   uint32_t a_box_bytes, b_box_bytes;
   // ---- epilogue
@@ -155,7 +161,7 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo1
 }
 
 // wgmma.mma_async m64nNk8 (tf32, K-major operands) / m64nNk16 (bf16; TR = 1: both operands MN-major), D += A * B.
-// The accumulator array is always 128 floats; an N-column instruction uses its first N / 2.
+// The accumulator array holds the instruction's N / 2 floats per thread.
 template <int DT, int TR>
 __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db) {
   if (DT == DT_TF32) {
@@ -169,7 +175,7 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_
   }
 }
 template <int DT, int TR>
-__device__ __forceinline__ void wgmma_n128(float (&d)[128], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db) {
   if (DT == DT_TF32) {
     asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1;"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
@@ -181,7 +187,7 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[128], uint64_t da, uint64_
   }
 }
 template <int DT, int TR>
-__device__ __forceinline__ void wgmma_n64(float (&d)[128], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db) {
   if (DT == DT_TF32) {
     asm volatile("wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1;"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
@@ -193,10 +199,11 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[128], uint64_t da, uint64_t
   }
 }
 
-template <int DT, int TR>
-__device__ __forceinline__ void wgmma_any(float (&d)[128], int ncols, uint64_t da, uint64_t db) {
-  if (ncols == 256) wgmma_n256<DT, TR>(d, da, db);
-  else if (ncols == 128) wgmma_n128<DT, TR>(d, da, db);
+template <int DT, int TR, int W>
+__device__ __forceinline__ void wgmma_tile(float (&d)[W / 2], uint64_t da, uint64_t db) {
+  static_assert(W == 64 || W == 128 || W == 256, "wgmma width");
+  if constexpr (W == 256) wgmma_n256<DT, TR>(d, da, db);
+  else if constexpr (W == 128) wgmma_n128<DT, TR>(d, da, db);
   else wgmma_n64<DT, TR>(d, da, db);
 }
 
@@ -234,43 +241,268 @@ __device__ __forceinline__ TileCoord tile_coord(const GemmParams& p, int u) {
   return c;
 }
 
-// tf32 weight gradient: the TMA lands both operands MN-major (rows = 32 pixels of 128 B = 32 channels, 128B swizzle,
-// one 4 KB box per 32 channels); wgmma needs tf32 K-major, so the 256 consumer threads rewrite the stage as
-// (128 + block_n) channel rows x 32 pixels (128 B, 128B swizzle) -- the layout of a K-major stage.
-__device__ __forceinline__ void transpose_stage_tf32(const uint8_t* src, uint8_t* dst, int rows, int ct) {
-  for (int gi = ct; gi < rows * 8; gi += 256) {
-    const int r = gi >> 3, kq = gi & 7;
-    const int region = r < 128 ? 0 : kStageABytes;
-    const int local = r < 128 ? r : r - 128;
-    const uint8_t* s = src + region + (local >> 5) * 4096;
-    const int c = local & 31;
-    float v[4];
+// tf32 weight gradient: the TMA lands both operands MN-major (a 4 KB box = 32 pixel rows of 128 B = 32 channels, 128B
+// swizzle; A = 4 boxes of dY channels, then B = BN / 32 boxes of X channels); wgmma takes tf32 K-major only, so the 8
+// consumer warps (w = 0..7) rewrite the stage as (128 + BN) channel rows x 32 pixels (128 B, 128B swizzle) -- the layout
+// of a K-major stage.  Work item = (box j, pixel quad q), lane = channel c of the box.  Banks:
+//   loads: element (pix, c) is at byte pix * 128 + (((c >> 2) ^ (pix & 7)) << 4) + (c & 3) * 4 of its box, so for one
+//          pix the 32 lanes hit banks ((c >> 2) ^ (pix & 7)) * 4 + (c & 3): all 32 distinct, one wavefront per load;
+//   store: lane c writes pixels 4q..4q+3 as 16 B to row r = 32 j + c, 16-byte chunk q ^ (r & 7); the 8 lanes of each
+//          quarter-warp phase have distinct r & 7, hence distinct chunks: the warp's 512 B take the minimum 4 wavefronts.
+// Each warp loads kBatch items before it stores them, so that several loads are in flight.
+template <int BN>
+__device__ __forceinline__ void transpose_stage_tf32(const uint8_t* src, uint8_t* dst, int w, int lane) {
+  constexpr int kItems = (128 + BN) / 32 * 8;
+  constexpr int kBatch = 4;
+  const int c = lane;
+  for (int it0 = w; it0 < kItems; it0 += 8 * kBatch) {
+    float v[kBatch][4];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int pix = kq * 4 + e;
-      v[e] = *reinterpret_cast<const float*>(s + pix * 128 + ((((c >> 2) ^ (pix & 7))) << 4) + (c & 3) * 4);
+    for (int b = 0; b < kBatch; ++b) {
+      const int it = it0 + 8 * b;
+      if (it < kItems) {
+        const uint8_t* box = src + (it >> 3) * 4096;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int pix = 4 * (it & 7) + e;
+          v[b][e] = *reinterpret_cast<const float*>(box + pix * 128 + (((c >> 2) ^ (pix & 7)) << 4) + (c & 3) * 4);
+        }
+      }
     }
-    *reinterpret_cast<float4*>(dst + region + local * 128 + ((kq ^ (local & 7)) << 4)) = make_float4(v[0], v[1], v[2], v[3]);
+#pragma unroll
+    for (int b = 0; b < kBatch; ++b) {
+      const int it = it0 + 8 * b;
+      if (it < kItems) {
+        const int r = 32 * (it >> 3) + c, q = it & 7;
+        *reinterpret_cast<float4*>(dst + r * 128 + ((q ^ (r & 7)) << 4)) = make_float4(v[b][0], v[b][1], v[b][2], v[b][3]);
+      }
+    }
+  }
+}
+
+// the shared-memory stages the consumers read (the TMA ring, or the K-major ring of a tf32 weight gradient)
+struct Ring {
+  uint8_t* base;
+  uint32_t stride;
+  int n;
+  uint64_t* full;   // completes when a stage holds operands
+  uint64_t* empty;  // one arrival per consumer warp when its wgmma have read the stage
+};
+
+// tf32 weight gradient: transpose the next TMA stage (raw ring position rs / rph) into the K-major ring at s / ph (the
+// stage the consumers read next), then hand the TMA stage back
+template <int BN>
+__device__ __forceinline__ void xpose_next(const Ring& raw, int& rs, uint32_t& rph, const Ring& ring, int s, uint32_t ph) {
+  const int lane = threadIdx.x & 31;
+  mbar_wait(&raw.full[rs], rph);
+  mbar_wait(&ring.empty[s], ph ^ 1u);   // both warpgroups' wgmma that read this K-major stage have completed
+  transpose_stage_tf32<BN>(raw.base + (size_t)rs * raw.stride, ring.base + (size_t)s * ring.stride,
+                           (threadIdx.x - 128) >> 5, lane);
+  fence_proxy_async();   // generic-proxy stores -> visible to the wgmma (async proxy) that read them
+  __syncwarp();
+  if (lane == 0) {
+    mbar_arrive(&raw.empty[rs]);
+    mbar_arrive(&ring.full[s]);
+  }
+  if (++rs == raw.n) { rs = 0; rph ^= 1u; }
+}
+
+// One work unit of W output columns (W = BN for a whole tile, PN for a column piece): mainloop, split-K parking and
+// epilogue.  s / ph: position in the ring, carried across units.  XP (tf32 weight gradient): the consumers read the
+// K-major ring and fill it themselves from the TMA ring (raw, position rs / rph): the transpose of stage i + 1 runs while
+// the tensor cores work on the wgmma of stage i.
+template <int DT, int TR, int W, bool XP>
+__device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoord& tc, const Ring& ring, int& s,
+                                             uint32_t& ph, const Ring& raw, int& rs, uint32_t& rph, float* st_buf,
+                                             int* bcast) {
+  const int ct = threadIdx.x - 128;          // 0..255
+  const int g = ct >> 7;
+  const int lane = threadIdx.x & 31;
+  const int wl = (ct >> 5) & 3;
+  const int cq = 2 * (lane & 3);             // first of the two columns this thread holds per 8-column block
+  const bool f_stats = p.stats != nullptr;
+  float acc[W / 2];
+#pragma unroll
+  for (int i = 0; i < W / 2; ++i) acc[i] = 0.f;
+  if constexpr (XP) {
+    if (tc.nkb > 0) xpose_next<W>(raw, rs, rph, ring, s, ph);
+  }
+  for (int i = 0; i < tc.nkb; ++i) {
+    mbar_wait(&ring.full[s], ph);
+    const uint32_t sa = smem_u32(ring.base + (size_t)s * ring.stride);
+    const uint32_t sb = sa + kStageABytes;
+    const uint64_t da = make_smem_desc(sa + (uint32_t)g * p.a_half, p.a_lbo, p.a_sbo);
+    const uint64_t db = make_smem_desc(sb, p.b_lbo, p.b_sbo);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kMmasPerKb; ++k)
+      wgmma_tile<DT, TR, W>(acc, da + (uint64_t)(k * p.a_kadv), db + (uint64_t)(k * p.b_kadv));
+    wgmma_commit();
+    // the previous k-block's wgmma have completed: hand its stage back
+    wgmma_wait<1>();
+    if (i > 0 && lane == 0) mbar_arrive(&ring.empty[s == 0 ? ring.n - 1 : s - 1]);
+    if (++s == ring.n) { s = 0; ph ^= 1u; }
+    if constexpr (XP) {
+      if (i + 1 < tc.nkb) xpose_next<W>(raw, rs, rph, ring, s, ph);
+    }
+  }
+  wgmma_wait<0>();
+  if (tc.nkb > 0 && lane == 0) mbar_arrive(&ring.empty[s == 0 ? ring.n - 1 : s - 1]);
+
+  // ---------------- split of a split-K tile: park the raw accumulators; the last split to arrive sums all of them
+  // in split order
+  if (tc.slice >= 0) {
+    const int nsl = p.splits;
+    float* ws = reinterpret_cast<float*>(p.tail_ws);
+    const size_t slice_elems = (size_t)128 * 256;
+    const size_t base = (size_t)tc.tail * nsl * slice_elems + ct;
+    float* dst = ws + base + (size_t)tc.slice * slice_elems;
+#pragma unroll
+    for (int i = 0; i < W / 2; ++i) dst[(size_t)i * 256] = acc[i];
+    __threadfence();
+    consumer_sync();
+    if (ct == 0) *bcast = atomicAdd(p.tail_cnt + tc.tail, 1);
+    consumer_sync();
+    const int old = *bcast;
+    if (old != nsl - 1) return;          // another slice finishes this tile
+    if (ct == 0) p.tail_cnt[tc.tail] = 0;       // self-cleaning for the next launch
+    __threadfence();
+    const float* src = ws + base;
+#pragma unroll
+    for (int i = 0; i < W / 2; ++i) {
+      float a = __ldcg(src + (size_t)i * 256);
+      for (int sl = 1; sl < nsl; ++sl) a += __ldcg(src + (size_t)sl * slice_elems + (size_t)i * 256);
+      acc[i] = a;
+    }
+  }
+
+  // ---------------- epilogue: this thread holds rows r0 and r0 + 8, columns 8 j + cq, 8 j + cq + 1
+  const int r0 = 64 * g + 16 * wl + (lane >> 2);
+  long row[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m_local = r0 + 8 * h;
+    if (p.mode == MODE_CONV) {
+      const int n_img = tc.tile_m / p.tiles_per_img;
+      const int r = tc.tile_m - n_img * p.tiles_per_img;
+      const int th = r / p.tiles_w;
+      const int oh = th * p.tile_h + m_local / p.tile_w;
+      const int ow = (r - th * p.tiles_w) * p.tile_w + m_local % p.tile_w;
+      row[h] = ((long)n_img * p.out_H + (long)oh * p.out_s + p.out_oh) * p.out_W + (long)ow * p.out_s + p.out_ow;
+      row_ok[h] = oh < p.Ho && ow < p.Wo;
+    } else {
+      row[h] = (long)tc.tile_m * 128 + m_local;
+      row_ok[h] = row[h] < p.M;
+    }
+  }
+  int col_base = tc.col0;
+  if (p.mode == MODE_WGRAD) {
+    const int tap = tc.tile_n / p.wg_cin_blocks;
+    col_base = tap * (p.wg_cin_blocks * p.block_n) + (tc.tile_n - tap * p.wg_cin_blocks) * p.block_n;
+  }
+  const __nv_bfloat16* res16 = reinterpret_cast<const __nv_bfloat16*>(p.residual);
+#pragma unroll
+  for (int j = 0; j < W / 8; ++j) {
+    const int n = col_base + 8 * j + cq;
+    float sm0 = 0.f, sm1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+    if (n < p.N) {
+      const bool two = n + 1 < p.N;
+      const float sc0 = p.scale ? __ldg(p.scale + n) : 1.f, sc1 = (p.scale && two) ? __ldg(p.scale + n + 1) : 1.f;
+      const float bi0 = p.bias ? __ldg(p.bias + n) : 0.f, bi1 = (p.bias && two) ? __ldg(p.bias + n + 1) : 0.f;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!row_ok[h]) continue;
+        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        if (p.scale) { x0 *= sc0; x1 *= sc1; }
+        if (p.bias) { x0 += bi0; x1 += bi1; }
+        const long ro = row[h];
+        if (p.residual) {
+          // bf16 output implies a bf16 residual (mixed-precision activations); fp32 otherwise
+          if (p.out_bf16) {
+            x0 += __bfloat162float(res16[ro * p.ldr + n]);
+            if (two) x1 += __bfloat162float(res16[ro * p.ldr + n + 1]);
+          } else {
+            x0 += p.residual[ro * p.ldr + n];
+            if (two) x1 += p.residual[ro * p.ldr + n + 1];
+          }
+        }
+        if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (p.out_bf16) {
+          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.C) + ro * p.ldc + n;
+          const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
+          x0 = __low2float(h2);   // statistics of the values the consumer reads
+          x1 = __high2float(h2);
+          if (two && (reinterpret_cast<uintptr_t>(o) & 3) == 0) *reinterpret_cast<__nv_bfloat162*>(o) = h2;
+          else { o[0] = __low2bfloat16(h2); if (two) o[1] = __high2bfloat16(h2); }
+        } else {
+          float* o = p.C + ro * p.ldc + n;
+          if (p.atomic) {
+            atomicAdd(o, x0);
+            if (two) atomicAdd(o + 1, x1);
+          } else if (two && (reinterpret_cast<uintptr_t>(o) & 7) == 0) {
+            *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
+          } else {
+            o[0] = x0;
+            if (two) o[1] = x1;
+          }
+        }
+        if (f_stats) {
+          sm0 += x0; sq0 = fmaf(x0, x0, sq0);
+          if (two) { sm1 += x1; sq1 = fmaf(x1, x1, sq1); }
+        }
+      }
+    }
+    if (f_stats) {
+      // column sums over the warp's 16 rows (lanes with equal lane & 3 hold the same columns), then over the CTA
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        sm0 += __shfl_xor_sync(0xffffffffu, sm0, o);
+        sm1 += __shfl_xor_sync(0xffffffffu, sm1, o);
+        sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
+        sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
+      }
+      if (lane < 4) {
+        // this warp's partial sums; summed over the 8 warps in a fixed order below (deterministic forward pass)
+        float* w = st_buf + (ct >> 5) * 512 + 8 * j + cq;
+        w[0] = sm0; w[1] = sm1; w[256] = sq0; w[257] = sq1;
+      }
+    }
+  }
+  if (f_stats) {
+    consumer_sync();
+    if (ct < W && col_base + ct < p.N) {
+      float a = 0.f, b = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) { a += st_buf[w * 512 + ct]; b += st_buf[w * 512 + 256 + ct]; }
+      if (a != 0.f || b != 0.f) {
+        atomicAdd(p.stats + col_base + ct, (double)a);
+        atomicAdd(p.stats + p.N + col_base + ct, (double)b);
+      }
+    }
+    consumer_sync();   // the slots are rewritten by the next tile
   }
 }
 
 // Persistent: each CTA walks work units blockIdx.x, blockIdx.x + gridDim.x, ...; the shared-memory ring runs across
 // tile boundaries, so the producer loads the next tile's operands while the consumers run this tile's epilogue.
-// MN = 1: WGRAD operands (MN-major).
-template <int DT, int MN>
+// MN = 1: WGRAD operands (MN-major).  BN: tile width; PN: width of a tail tile's column pieces (0: no pieces).
+template <int DT, int MN, int BN, int PN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const __grid_constant__ CUtensorMap tma_bp, const __grid_constant__ GemmParams p) {
   constexpr bool kXpose = MN == 1 && DT == DT_TF32;
+  constexpr uint32_t kStageBytes = kStageABytes + BN * 128u;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages x (A 16KB | B block_n*128B)] | [tf32 WGRAD: one K-major stage] | statistics 16 KB | barriers
+  // carve: [stages x (A 16KB | B BN*128B)] | [tf32 WGRAD: kXStages K-major stages] | statistics 16 KB | barriers
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const uint32_t stage_bytes = kStageABytes + (uint32_t)p.block_n * 128u;
-  uint8_t* xbuf = smem + (size_t)p.stages * stage_bytes;
-  float* st_buf = reinterpret_cast<float*>(xbuf + (kXpose ? stage_bytes : 0u));
+  uint8_t* xbuf = smem + (size_t)p.stages * kStageBytes;
+  float* st_buf = reinterpret_cast<float*>(xbuf + (kXpose ? kXStages * kStageBytes : 0u));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(st_buf) + kStatsBytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  int* bcast = reinterpret_cast<int*>(empty_bar + p.stages);
+  uint64_t* xfull_bar = empty_bar + p.stages;     // K-major ring of a tf32 weight gradient
+  uint64_t* xempty_bar = xfull_bar + kXStages;
+  int* bcast = reinterpret_cast<int*>(xempty_bar + kXStages);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_whole = p.tiles_m * p.tiles_n * p.splits;
@@ -280,10 +512,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-    if (p.tail_p > 0) tma_prefetch_desc(&tma_bp);
+    if (PN > 0 && p.tail_p > 0) tma_prefetch_desc(&tma_bp);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
+    }
+    if (kXpose) {
+      for (int s = 0; s < kXStages; ++s) {
+        mbar_init(&xfull_bar[s], 8);
+        mbar_init(&xempty_bar[s], 8);
+      }
     }
     fence_barrier_init();
   }
@@ -315,7 +553,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         }
         for (int i = 0; i < tc.nkb; ++i) {
           mbar_wait(&empty_bar[s], ph ^ 1u);
-          uint8_t* sa = smem + (size_t)s * stage_bytes;
+          uint8_t* sa = smem + (size_t)s * kStageBytes;
           uint8_t* sb = sa + kStageABytes;
           const int kb = tc.split * p.num_kb + tc.kb0 + i;
           if (!leader) {
@@ -352,190 +590,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
 
   // =============================== consumers: warpgroup g = 0 / 1 owns rows 64 g .. 64 g + 63 of the tile
   setmaxnreg_inc<232>();
-  const int ct = threadIdx.x - 128;          // 0..255
-  const int g = ct >> 7;
-  const int wl = (ct >> 5) & 3;
-  const int cq = 2 * (lane & 3);             // first of the two columns this thread holds per 8-column block
-  const bool f_stats = p.stats != nullptr;
-  int s = 0;
-  uint32_t ph = 0;
+  const Ring raw{smem, kStageBytes, p.stages, full_bar, empty_bar};
+  const Ring ring = kXpose ? Ring{xbuf, kStageBytes, kXStages, xfull_bar, xempty_bar} : raw;
+  constexpr int kTR = kXpose ? 0 : MN;
+  int s = 0, rs = 0;
+  uint32_t ph = 0, rph = 0;
   for (int t = blockIdx.x; t < total_units; t += gridDim.x) {
     const TileCoord tc = tile_coord(p, t);
-    const int ncols = tc.ncols;
-    float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    for (int i = 0; i < tc.nkb; ++i) {
-      mbar_wait(&full_bar[s], ph);
-      uint32_t sa, sb;
-      if (kXpose) {
-        consumer_sync();   // both warpgroups' wgmma of the previous k-block (which read xbuf) have completed
-        transpose_stage_tf32(smem + (size_t)s * stage_bytes, xbuf, 128 + p.block_n, ct);
-        fence_proxy_async();
-        consumer_sync();
-        if (lane == 0) mbar_arrive(&empty_bar[s]);
-        sa = smem_u32(xbuf);
-      } else {
-        sa = smem_u32(smem + (size_t)s * stage_bytes);
-      }
-      sb = sa + kStageABytes;
-      const uint64_t da = make_smem_desc(sa + (uint32_t)g * p.a_half, p.a_lbo, p.a_sbo);
-      const uint64_t db = make_smem_desc(sb, p.b_lbo, p.b_sbo);
-      wgmma_fence();
-      for (int k = 0; k < p.mmas_per_kb; ++k)
-        wgmma_any<DT, kXpose ? 0 : MN>(acc, ncols, da + (uint64_t)(k * p.a_kadv), db + (uint64_t)(k * p.b_kadv));
-      wgmma_commit();
-      if (kXpose) {
-        wgmma_wait<0>();
-      } else {
-        // the previous k-block's wgmma have completed: hand its stage back to the producer
-        wgmma_wait<1>();
-        if (i > 0 && lane == 0) mbar_arrive(&empty_bar[s == 0 ? p.stages - 1 : s - 1]);
-      }
-      if (++s == p.stages) { s = 0; ph ^= 1u; }
-    }
-    if (!kXpose) {
-      wgmma_wait<0>();
-      if (tc.nkb > 0 && lane == 0) mbar_arrive(&empty_bar[s == 0 ? p.stages - 1 : s - 1]);
-    }
-
-    // ---------------- split of a split-K tile: park the raw accumulators; the last split to arrive sums all of them
-    // in split order
-    if (tc.slice >= 0) {
-      const int nsl = p.splits;
-      float* ws = reinterpret_cast<float*>(p.tail_ws);
-      const size_t slice_elems = (size_t)128 * 256;
-      const size_t base = (size_t)tc.tail * nsl * slice_elems + ct;
-      float* dst = ws + base + (size_t)tc.slice * slice_elems;
-#pragma unroll
-      for (int i = 0; i < 128; ++i)
-        if (i < ncols / 2) dst[(size_t)i * 256] = acc[i];
-      __threadfence();
-      consumer_sync();
-      if (ct == 0) *bcast = atomicAdd(p.tail_cnt + tc.tail, 1);
-      consumer_sync();
-      const int old = *bcast;
-      if (old != nsl - 1) continue;          // another slice finishes this tile
-      if (ct == 0) p.tail_cnt[tc.tail] = 0;       // self-cleaning for the next launch
-      __threadfence();
-      const float* src = ws + base;
-#pragma unroll
-      for (int i = 0; i < 128; ++i) {
-        if (i < ncols / 2) {
-          float a = __ldcg(src + (size_t)i * 256);
-          for (int sl = 1; sl < nsl; ++sl) a += __ldcg(src + (size_t)sl * slice_elems + (size_t)i * 256);
-          acc[i] = a;
-        }
+    if constexpr (PN > 0) {
+      if (tc.piece) {
+        consume_unit<DT, kTR, PN, false>(p, tc, ring, s, ph, raw, rs, rph, st_buf, bcast);
+        continue;
       }
     }
-
-    // ---------------- epilogue: this thread holds rows r0 and r0 + 8, columns 8 j + cq, 8 j + cq + 1
-    const int r0 = 64 * g + 16 * wl + (lane >> 2);
-    long row[2];
-    bool row_ok[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m_local = r0 + 8 * h;
-      if (p.mode == MODE_CONV) {
-        const int n_img = tc.tile_m / p.tiles_per_img;
-        const int r = tc.tile_m - n_img * p.tiles_per_img;
-        const int th = r / p.tiles_w;
-        const int oh = th * p.tile_h + m_local / p.tile_w;
-        const int ow = (r - th * p.tiles_w) * p.tile_w + m_local % p.tile_w;
-        row[h] = ((long)n_img * p.out_H + (long)oh * p.out_s + p.out_oh) * p.out_W + (long)ow * p.out_s + p.out_ow;
-        row_ok[h] = oh < p.Ho && ow < p.Wo;
-      } else {
-        row[h] = (long)tc.tile_m * 128 + m_local;
-        row_ok[h] = row[h] < p.M;
-      }
-    }
-    int col_base = tc.col0;
-    if (p.mode == MODE_WGRAD) {
-      const int tap = tc.tile_n / p.wg_cin_blocks;
-      col_base = tap * (p.wg_cin_blocks * p.block_n) + (tc.tile_n - tap * p.wg_cin_blocks) * p.block_n;
-    }
-    const __nv_bfloat16* res16 = reinterpret_cast<const __nv_bfloat16*>(p.residual);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      if (8 * j >= ncols) break;
-      const int n = col_base + 8 * j + cq;
-      float sm0 = 0.f, sm1 = 0.f, sq0 = 0.f, sq1 = 0.f;
-      if (n < p.N) {
-        const bool two = n + 1 < p.N;
-        const float sc0 = p.scale ? __ldg(p.scale + n) : 1.f, sc1 = (p.scale && two) ? __ldg(p.scale + n + 1) : 1.f;
-        const float bi0 = p.bias ? __ldg(p.bias + n) : 0.f, bi1 = (p.bias && two) ? __ldg(p.bias + n + 1) : 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!row_ok[h]) continue;
-          float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-          if (p.scale) { x0 *= sc0; x1 *= sc1; }
-          if (p.bias) { x0 += bi0; x1 += bi1; }
-          const long ro = row[h];
-          if (p.residual) {
-            // bf16 output implies a bf16 residual (mixed-precision activations); fp32 otherwise
-            if (p.out_bf16) {
-              x0 += __bfloat162float(res16[ro * p.ldr + n]);
-              if (two) x1 += __bfloat162float(res16[ro * p.ldr + n + 1]);
-            } else {
-              x0 += p.residual[ro * p.ldr + n];
-              if (two) x1 += p.residual[ro * p.ldr + n + 1];
-            }
-          }
-          if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-          if (p.out_bf16) {
-            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.C) + ro * p.ldc + n;
-            const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
-            x0 = __low2float(h2);   // statistics of the values the consumer reads
-            x1 = __high2float(h2);
-            if (two && (reinterpret_cast<uintptr_t>(o) & 3) == 0) *reinterpret_cast<__nv_bfloat162*>(o) = h2;
-            else { o[0] = __low2bfloat16(h2); if (two) o[1] = __high2bfloat16(h2); }
-          } else {
-            float* o = p.C + ro * p.ldc + n;
-            if (p.atomic) {
-              atomicAdd(o, x0);
-              if (two) atomicAdd(o + 1, x1);
-            } else if (two && (reinterpret_cast<uintptr_t>(o) & 7) == 0) {
-              *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
-            } else {
-              o[0] = x0;
-              if (two) o[1] = x1;
-            }
-          }
-          if (f_stats) {
-            sm0 += x0; sq0 = fmaf(x0, x0, sq0);
-            if (two) { sm1 += x1; sq1 = fmaf(x1, x1, sq1); }
-          }
-        }
-      }
-      if (f_stats) {
-        // column sums over the warp's 16 rows (lanes with equal lane & 3 hold the same columns), then over the CTA
-#pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          sm0 += __shfl_xor_sync(0xffffffffu, sm0, o);
-          sm1 += __shfl_xor_sync(0xffffffffu, sm1, o);
-          sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
-          sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
-        }
-        if (lane < 4) {
-          // this warp's partial sums; summed over the 8 warps in a fixed order below (deterministic forward pass)
-          float* w = st_buf + (ct >> 5) * 512 + 8 * j + cq;
-          w[0] = sm0; w[1] = sm1; w[256] = sq0; w[257] = sq1;
-        }
-      }
-    }
-    if (f_stats) {
-      consumer_sync();
-      if (ct < ncols && col_base + ct < p.N) {
-        float a = 0.f, b = 0.f;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) { a += st_buf[w * 512 + ct]; b += st_buf[w * 512 + 256 + ct]; }
-        if (a != 0.f || b != 0.f) {
-          atomicAdd(p.stats + col_base + ct, (double)a);
-          atomicAdd(p.stats + p.N + col_base + ct, (double)b);
-        }
-      }
-      consumer_sync();   // the slots are rewritten by the next tile
-    }
+    consume_unit<DT, kTR, BN, kXpose>(p, tc, ring, s, ph, raw, rs, rph, st_buf, bcast);
   }
 }
 
@@ -580,16 +648,16 @@ int make_map(CUtensorMap* m, int dtype, const void* base, const uint64_t dims[4]
 constexpr int kSmemMax = 227 * 1024;       // opt-in dynamic shared memory per block (H100)
 constexpr int kSmemFixed = 1024 + kStatsBytes + 512;   // alignment slack, statistics, barriers
 
-// one persistent CTA per SM: fill shared memory with the operand ring (tf32 weight gradients also keep one K-major
-// stage for the transposed operands)
+// one persistent CTA per SM: fill shared memory with the operand ring (tf32 weight gradients also keep kXStages
+// K-major stages for the transposed operands; at block_n = 256 that leaves a 2-stage TMA ring)
 int pick_stages(int block_n, int xpose = 0) {
   const int stage = kStageABytes + block_n * 128;
-  int s = (kSmemMax - kSmemFixed) / stage - (xpose ? 1 : 0);
+  int s = (kSmemMax - kSmemFixed) / stage - (xpose ? kXStages : 0);
   return s > 8 ? 8 : s;
 }
 
 size_t smem_bytes(int stages, int block_n, int xpose) {
-  return (size_t)(stages + (xpose ? 1 : 0)) * (kStageABytes + block_n * 128) + kSmemFixed;
+  return (size_t)(stages + (xpose ? kXStages : 0)) * (kStageABytes + block_n * 128) + kSmemFixed;
 }
 
 // Split-K workspaces: kTailSlots buffers per device (one per stream using the kernel concurrently) carved out of
@@ -680,20 +748,36 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmParams& p, dim3 til
   const int xpose = (p.mode == MODE_WGRAD && p.dtype == DT_TF32) ? 1 : 0;
   const size_t smem = smem_bytes(p.stages, p.block_n, xpose);
   typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmParams);
-  // [operand type][MN-major operands]
-  static const KernelFn kernels[2][2] = {{gemm_tc_kernel<DT_TF32, 0>, gemm_tc_kernel<DT_TF32, 1>},
-                                         {gemm_tc_kernel<DT_BF16, 0>, gemm_tc_kernel<DT_BF16, 1>}};
+  // every instantiation: operand type, MN-major operands, tile width, column-piece width (tail splits of 256-wide
+  // K-major tiles only)
+  struct Instance { int dt, mn, bn, pn; KernelFn fn; };
+  static const Instance kernels[] = {
+      {DT_TF32, 0, 64, 0, gemm_tc_kernel<DT_TF32, 0, 64, 0>},     {DT_TF32, 0, 128, 0, gemm_tc_kernel<DT_TF32, 0, 128, 0>},
+      {DT_TF32, 0, 256, 0, gemm_tc_kernel<DT_TF32, 0, 256, 0>},   {DT_TF32, 0, 256, 64, gemm_tc_kernel<DT_TF32, 0, 256, 64>},
+      {DT_TF32, 0, 256, 128, gemm_tc_kernel<DT_TF32, 0, 256, 128>},
+      {DT_TF32, 1, 64, 0, gemm_tc_kernel<DT_TF32, 1, 64, 0>},     {DT_TF32, 1, 128, 0, gemm_tc_kernel<DT_TF32, 1, 128, 0>},
+      {DT_TF32, 1, 256, 0, gemm_tc_kernel<DT_TF32, 1, 256, 0>},
+      {DT_BF16, 0, 64, 0, gemm_tc_kernel<DT_BF16, 0, 64, 0>},     {DT_BF16, 0, 128, 0, gemm_tc_kernel<DT_BF16, 0, 128, 0>},
+      {DT_BF16, 0, 256, 0, gemm_tc_kernel<DT_BF16, 0, 256, 0>},   {DT_BF16, 0, 256, 64, gemm_tc_kernel<DT_BF16, 0, 256, 64>},
+      {DT_BF16, 0, 256, 128, gemm_tc_kernel<DT_BF16, 0, 256, 128>},
+      {DT_BF16, 1, 64, 0, gemm_tc_kernel<DT_BF16, 1, 64, 0>},     {DT_BF16, 1, 128, 0, gemm_tc_kernel<DT_BF16, 1, 128, 0>},
+      {DT_BF16, 1, 256, 0, gemm_tc_kernel<DT_BF16, 1, 256, 0>}};
+  constexpr int kNumKernels = (int)(sizeof(kernels) / sizeof(kernels[0]));
   // per-device one-time setup (a process may drive several GPUs)
   static bool attr_done[64] = {false};
   int dev = 0;
   SN_CUDA(cudaGetDevice(&dev));
   if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b)
-        SN_CUDA(cudaFuncSetAttribute(kernels[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    for (int i = 0; i < kNumKernels; ++i)
+      SN_CUDA(cudaFuncSetAttribute(kernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     attr_done[dev] = true;
   }
-  KernelFn fn = kernels[p.dtype == DT_TF32 ? 0 : 1][p.mode == MODE_WGRAD ? 1 : 0];
+  const int mn = p.mode == MODE_WGRAD ? 1 : 0, pn = p.tail_p > 0 ? p.block_n / p.tail_p : 0;
+  KernelFn fn = nullptr;
+  for (int i = 0; i < kNumKernels; ++i)
+    if (kernels[i].dt == p.dtype && kernels[i].mn == mn && kernels[i].bn == p.block_n && kernels[i].pn == pn)
+      fn = kernels[i].fn;
+  SN_CHECK(fn != nullptr, "gemm: no kernel for block_n %d with %d-column tail pieces", p.block_n, pn);
   const unsigned grid = (unsigned)(units < max_units ? units : max_units);
   fn<<<grid, kThreads, smem, stream>>>(ma, mb, mbp, p);
   SN_LAUNCH_CHECK();
@@ -724,7 +808,6 @@ void fill_kmajor(GemmParams& p, int dtype, int block_n) {
   p.a_lbo = 1; p.a_sbo = 64; p.b_lbo = 1; p.b_sbo = 64;
   p.a_kadv = 2; p.b_kadv = 2;
   p.a_half = 64 * 128;                                   // the second consumer's rows 64..127
-  p.mmas_per_kb = 4;
   p.a_boxes = 1; p.b_boxes = 1;
   p.a_box_bytes = kStageABytes;
   p.b_box_bytes = (uint32_t)block_n * 128u;
@@ -874,15 +957,13 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
     p.a_lbo = 1; p.a_sbo = 64; p.b_lbo = 1; p.b_sbo = 64;
     p.a_kadv = 2; p.b_kadv = 2;
     p.a_half = 64 * 128;
-    p.mmas_per_kb = 4;
   } else {
     // MN-major, 128B swizzle: LBO = stride between 64-element MN atoms (one TMA box of kp pixel rows), SBO = stride
-    // between 8-pixel-row groups; one wgmma consumes 16 pixel rows (2 KB); the second consumer's 64 output channels
-    // are the second box of A
+    // between 8-pixel-row groups; one wgmma consumes 16 pixel rows (2 KB), kMmasPerKb of them the kp = 64 pixels of a
+    // k-block; the second consumer's 64 output channels are the second box of A
     p.a_lbo = chunk_bytes >> 4; p.a_sbo = 64; p.b_lbo = chunk_bytes >> 4; p.b_sbo = 64;
     p.a_kadv = (16 * 128) >> 4; p.b_kadv = p.a_kadv;
     p.a_half = chunk_bytes;
-    p.mmas_per_kb = kp / 16;
   }
   p.a_boxes = 128 / E; p.b_boxes = bn / E;
   p.a_box_bytes = chunk_bytes; p.b_box_bytes = chunk_bytes;
