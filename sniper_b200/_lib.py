@@ -24,9 +24,6 @@ SIGNATURES = {
     "sniper_deform_psroi_fwd": ("i", "ppp" "iiii" "f" "iiiii" "f" "iii" "ppp" "p"),
     "sniper_deform_psroi_bwd": ("i", "pppp" "iiii" "f" "iiiii" "f" "iii" "pp" "p"),
     "sniper_deform_psroi_bwd_fp64acc": ("i", "pppp" "iiiii" "f" "iiiii" "f" "ii" "pp" "pl" "p"),
-    "sniper_deform_psroi_fwd_tiled": ("i", "ppp" "iiiii" "f" "iiiii" "f" "ii" "pp" "p"),
-    "sniper_deform_psroi_bwd_tiled_workspace_bytes": ("z", "iiii"),
-    "sniper_deform_psroi_bwd_tiled": ("i", "pppp" "iiiii" "f" "iiiii" "f" "ii" "pp" "pz" "p"),
     "sniper_psroi_fwd": ("i", "pp" "iiii" "f" "iiii" "pp" "p"),
     "sniper_psroi_bwd": ("i", "pp" "iiii" "f" "iiii" "p" "p"),
     "sniper_gemm_nt": ("i", "plplpl" "iiii" "ppp" "l" "iii" "pp"),
@@ -86,7 +83,7 @@ _lib = None
 KERNELS_PER_CALL = {
     "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
-    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_deform_psroi_bwd_tiled_workspace_bytes": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
+    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
 }
 launches = [0]

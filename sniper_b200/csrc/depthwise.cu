@@ -9,7 +9,6 @@
 // depthwise_convolution_tf.cuh), elemwise_add, im2col of nn/convolution-inl.h for the 3-channel first layer.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "depthwise_core.cuh"
@@ -48,11 +47,9 @@ int launch_fwd_tiled(const void* x, const float* w, void* y, const dwc::Params& 
   return 0;
 }
 
-// SNIPER_DW_TILED=0 selects the register-window kernels for bf16 too (A/B runs)
+// the tiled kernel takes bf16 with whole 64-channel groups; fp32 and other shapes run the register-window kernels
 bool use_tiled(int dtype, int C, long ld_in) {
-  static int flag = -1;
-  if (flag < 0) { const char* e = getenv("SNIPER_DW_TILED"); flag = (e && e[0] == '0') ? 0 : 1; }
-  return flag == 1 && dtype == 1 && C % 64 == 0 && ld_in % 8 == 0;       // 16-byte aligned pixel rows for cp.async
+  return dtype == 1 && C % 64 == 0 && ld_in % 8 == 0;       // 16-byte aligned pixel rows for cp.async
 }
 
 template <typename T>

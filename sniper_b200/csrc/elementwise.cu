@@ -7,13 +7,8 @@
 // smooth_l1 + MakeLoss (mshadow_op.h:642-678), SGD momentum (optimizer_op-inl.h:279-300).
 // All kernels: 128-bit vectorised loads/stores along C, grids sized in multiples of the SM count.
 #include "common.cuh"
-#include <cooperative_groups.h>
-#include <string.h>
-#include <stdlib.h>
 #include <cuda_bf16.h>
 #include <math.h>
-
-namespace cg = cooperative_groups;
 
 namespace {
 
@@ -289,11 +284,9 @@ __global__ void __launch_bounds__(256) colsum_kernel(const T* __restrict__ x, lo
       }
     }
   }
-  // Block partials -> cluster partials -> one double atomic per (cluster, channel, sum).  The row blocks of one channel
-  // slab are launched as thread-block clusters along x; rank 0 gathers the other blocks' partials through distributed
-  // shared memory.  Without this step every block issued its own atomics: ~600 same-address double atomics per channel
-  // for a 20480-row tensor, and their serialisation in L2 -- not the loads -- set the kernel time (it GREW with the
-  // block count: 15.6 / 19.1 / 40.8 us at 2 / 8 / 16 blocks per SM for 20480 x 256 fp32, tools/ew_time.py).
+  // Block partials, summed in a fixed thread order -> one double atomic per (block, channel, sum).  Same-address double
+  // atomics serialise in L2 and can set the kernel time (it grows with the block count), so row_block keeps the grid to
+  // one wave.
   __shared__ float sa[256][N + 1], sb[256][N + 1];
   __shared__ double part[2][32 * N];
 #pragma unroll
@@ -312,24 +305,17 @@ __global__ void __launch_bounds__(256) colsum_kernel(const T* __restrict__ x, lo
       part[1][threadIdx.x * N + k] = bx;
     }
   }
-  cg::cluster_group cluster = cg::this_cluster();
-  const unsigned nblk = cluster.num_blocks();
-  if (nblk > 1) cluster.sync(); else __syncthreads();
-  if (cluster.block_rank() == 0) {
-    const int per = lx * N;                  // channels of this slab
-    const int cbase = (int)blockIdx.y * per;
-    for (int i = threadIdx.x; i < 2 * per; i += 256) {
-      const int which = i >= per ? 1 : 0, j = i - which * per;
-      if (cbase + j >= C) continue;
-      double t = part[which][j];
-      for (unsigned r = 1; r < nblk; ++r) t += cluster.map_shared_rank(&part[0][0], r)[which * 32 * N + j];
-      if (t != 0.0) atomicAdd(sums + which * C + cbase + j, t);
-    }
+  __syncthreads();
+  const int per = lx * N;                    // channels of this slab
+  const int cbase = (int)blockIdx.y * per;
+  for (int i = threadIdx.x; i < 2 * per; i += 256) {
+    const int which = i >= per ? 1 : 0, j = i - which * per;
+    if (cbase + j >= C) continue;
+    const double t = part[which][j];
+    if (t != 0.0) atomicAdd(sums + which * C + cbase + j, t);
   }
-  if (nblk > 1) cluster.sync();              // keep every block's shared memory alive until rank 0 has read it
 }
 
-// Launches colsum_kernel with its row blocks grouped into thread-block clusters (SNIPER_EW_CLUSTER = 1 | 2 | 4 | 8, A/B).
 RowBlock row_block(long M, int C, int vec, int occ);
 template <typename K> int resident_blocks(K kernel);
 
@@ -337,24 +323,9 @@ template <int MODE, typename T>
 int launch_colsum(cudaStream_t st, const T* x, long ldx, const T* dy, long lddy, const float* scale,
                   const float* shift, const float* mean, const float* invstd, long M, int C, double* sums) {
   const RowBlock rb = row_block(M, C, VT<T>::N, resident_blocks(colsum_kernel<MODE, T>));
-  int cl = 1;   // measured: clusters only help the smallest tensors and cost 20-30 % on the large ones
-  if (const char* e = getenv("SNIPER_EW_CLUSTER")) cl = atoi(e);
-  if (cl != 1 && cl != 2 && cl != 4 && cl != 8) cl = 1;
-  while (cl > 1 && rb.grid.x < (unsigned)cl) cl >>= 1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((rb.grid.x + cl - 1) / cl * cl, rb.grid.y, 1);    // padding blocks own no rows
-  cfg.blockDim = dim3(256, 1, 1);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)cl;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = cl > 1 ? 1 : 0;
-  SN_CUDA(cudaLaunchKernelEx(&cfg, colsum_kernel<MODE, T>, x, ldx, dy, lddy, scale, shift, mean, invstd, M, C,
-                             rb.lx_shift, rb.rows_per_block, sums));
+  colsum_kernel<MODE, T><<<rb.grid, 256, 0, st>>>(x, ldx, dy, lddy, scale, shift, mean, invstd, M, C, rb.lx_shift,
+                                                  rb.rows_per_block, sums);
+  SN_LAUNCH_CHECK();
   return 0;
 }
 
@@ -864,14 +835,13 @@ int ew_grid(long work) {
 // API, cached per kernel); the rows are cut so that every slab's row blocks together fill <= kNumSMs * occ slots.  Sizing the
 // grid independently of the kernel's occupancy cost up to 2x: e.g. 640 blocks of the bf16 reduction kernel (2 resident
 // blocks per SM = 296 slots) ran as three waves of latency-bound blocks (tools/ew_time.py: 20480 x 256 bf16 backward
-// 47 us for 52 MB).  SNIPER_EW_BPS=<n> overrides occ (A/B runs).
+// 47 us for 52 MB).
 RowBlock row_block(long M, int C, int vec, int occ) {
   RowBlock rb;
   const int cv = C / vec;                       // vectors per row
   rb.lx_shift = cv >= 32 ? 5 : (cv >= 16 ? 4 : 3);
   const int lx = 1 << rb.lx_shift, RY = 256 >> rb.lx_shift;
   const int by = sn::div_up(cv, lx);
-  if (const char* e = getenv("SNIPER_EW_BPS")) occ = atoi(e) > 0 ? atoi(e) : occ;
   if (occ < 1) occ = 1;
   long slots = (long)sn::kNumSMs * occ - by;    // ceil() of the row split can add one block per slab
   if (slots < by) slots = by;

@@ -712,13 +712,8 @@ void plan_tail(GemmParams& p, long tiles, long grid_units) {
   if (tail == 0 || tail * 2 > grid_units) return;
   if (p.block_n == 256 && tiles > grid_units) {
     // column pieces: 4 x 64 columns if they fit one wave, else 2 x 128
-    long pcs = tail * 4 <= grid_units ? 4 : 2;
-    if (const char* m = getenv("SNIPER_GEMM_TAIL_MAXP")) pcs = pcs < atoi(m) ? pcs : atoi(m);
-    if (pcs >= 2) {
-      p.tail_p = (int)pcs;
-      p.tail_first = (int)(tiles - tail);
-      return;
-    }
+    p.tail_p = tail * 4 <= grid_units ? 4 : 2;
+    p.tail_first = (int)(tiles - tail);
   }
 }
 
@@ -785,17 +780,9 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmParams& p, dim3 til
 }
 
 // Tile width: wide tiles move fewer L2 -> shared-memory bytes per flop (a 128 x 128 tile moves 1.33x the bytes per
-// flop of a 128 x 256 tile), so 256 columns wherever N allows it.  SNIPER_GEMM_BN=<64|128|256> forces a width.
-int pick_block_n(int N, long tiles_m) {
-  (void)tiles_m;
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("SNIPER_GEMM_BN");
-    forced = e ? atoi(e) : 0;
-  }
-  const int cap = N <= 64 ? 64 : (N <= 128 ? 128 : 256);
-  if (forced == 64 || forced == 128 || forced == 256) return forced < cap ? forced : cap;
-  if (N <= 128) return cap;
+// flop of a 128 x 256 tile), so 256 columns wherever N allows it.
+int pick_block_n(int N) {
+  if (N <= 128) return N <= 64 ? 64 : 128;
   if (N % 256 == 0 || N > 1024) return 256;
   return 128;
 }
@@ -842,7 +829,7 @@ int sniper_gemm_nt(const void* A, long lda, const void* B, long ldb, float* C, l
   SN_CHECK((lda * esz) % 16 == 0 && (ldb * esz) % 16 == 0, "gemm: row strides must be 16-byte multiples");
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  const int bn = pick_block_n(N, sn::div_up(M, 128));
+  const int bn = pick_block_n(N);
   fill_kmajor(p, dtype, bn);
   p.mode = MODE_GEMM; p.M = M; p.N = N; p.num_kb = K / E;
   p.C = C; p.ldc = ldc; p.scale = scale; p.bias = bias; p.residual = residual; p.ldr = ldr; p.relu = relu;
@@ -891,7 +878,7 @@ int sniper_conv2d_nhwc(const void* X, long x_ld, int NB, int H, int W, int Cin, 
   SN_CHECK(tile_w * stride <= 256, "conv: TMA box too wide");
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  const int bn = pick_block_n(Cout, (long)NB * (Wo / tile_w) * sn::div_up(Ho, tile_h));
+  const int bn = pick_block_n(Cout);
   fill_kmajor(p, dtype, bn);
   p.mode = MODE_CONV; p.N = Cout; p.cblocks = Cin / E; p.ntaps = ntaps; p.num_kb = ntaps * p.cblocks;
   for (int t = 0; t < ntaps; ++t) { p.tap_dh[t] = tap_dh[t]; p.tap_dw[t] = tap_dw[t]; }
@@ -1048,7 +1035,7 @@ int sniper_gemm_plan(int M, int N, int K, int dtype, int* out) {
   SN_CHECK(M > 0 && N > 0 && K > 0 && K % E == 0, "gemm_plan: K (%d) must be a positive multiple of %d", K, E);
   GemmParams p;
   memset(&p, 0, sizeof(p));
-  const int bn = pick_block_n(N, sn::div_up(M, 128));
+  const int bn = pick_block_n(N);
   fill_kmajor(p, dtype, bn);
   p.mode = MODE_GEMM; p.M = M; p.N = N; p.num_kb = K / E;
   p.splits = 1;

@@ -548,183 +548,6 @@ int grid_for(long count) {
   return (int)(g > cap ? cap : (g < 1 ? 1 : g));
 }
 
-
-// ------------------------------------------------------------------------------------------------------------------
-// Chip-tiled kernels (NHWC, group_size 1): one CTA = one chip x 16 channels.  The chip's feature slice (forward) or
-// gradient slice (backward) lives in shared memory as [H*W][16 + 1 pad] floats, a warp walks the chip's ROIs with one
-// lane per bin, and
-//   forward : every bilinear gather is a shared-memory read (the warp-per-bin kernel above issued one 128-byte global
-//             gather per pixel and channel group and ran at ~10 % of the DRAM roof, bound by L1/L2 gather throughput);
-//   backward: the scatter is a shared-memory atomic and the slice is added to data_diff ONCE at the end with plain
-//             coalesced accesses -- no global atomics (the warp-per-bin kernel issued ~5.8 M warp-wide float4 REDs into a
-//             21 MB tensor per call and was bound by L2 atomic throughput: 0.85 ms per call).
-// The bin geometry is recomputed per channel slice (16 x per bin): ~200 instructions against 9 x 16 x 2 shared-memory
-// operations, and it keeps the kernels free of any intermediate table.  d(trans) needs the dot product over ALL channels:
-// every slice writes its partial (tdx, tdy) per bin to a caller-provided workspace and trans_reduce_kernel sums them.
-// Forward results are bit-identical to deform_psroi_fwd_sep_nhwc_kernel (same operation order per channel).
-// Not measured on the H100.  Expected to be slower than the warp-per-bin
-// kernels -- with one lane per bin a warp's shared-memory accesses scatter over pixels (bank conflicts; float atomics on
-// shared memory are compare-and-swap loops), which costs more than the global gathers / REDs it removes.  Kept as an
-// opt-in variant (ops: SNIPER_PSROI_TILED=1) with its parity test; the product path uses the warp-per-bin kernels.
-constexpr int kTileCh = 16;
-constexpr int kTilePad = kTileCh + 1;   // odd stride: pixels map to different banks
-
-template <bool BWD>
-__global__ void __launch_bounds__(256) deform_psroi_tiled_kernel(PsArgs p, float* __restrict__ trans_part) {
-  extern __shared__ float tile[];
-  const int slice = blockIdx.x, b = blockIdx.y;
-  const int c0 = slice * kTileCh;
-  const int HW = p.height * p.width;
-  const int C = p.channels;
-  if (!BWD) {
-    const float* img = p.data + (size_t)b * HW * C + c0;
-    for (int i = threadIdx.x; i < HW * 4; i += blockDim.x) {
-      const int px = i >> 2, q = i & 3;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(img + (size_t)px * C) + q);
-      float* t = tile + px * kTilePad + q * 4;
-      t[0] = v.x; t[1] = v.y; t[2] = v.z; t[3] = v.w;
-    }
-  } else {
-    for (int i = threadIdx.x; i < HW * kTilePad; i += blockDim.x) tile[i] = 0.f;
-  }
-  __syncthreads();
-  const int S = p.sample_per_part;
-  const int PP = p.pooled * p.pooled;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const long nbins = (long)p.num_rois * PP;
-  for (int n = warp; n < p.num_rois; n += nwarps) {
-    if ((int)p.rois[(size_t)n * 5] != b) continue;            // warp-uniform: this ROI belongs to another chip
-    for (int k = lane; k < PP; k += 32) {
-      const int ph = k / p.pooled, pw = k - ph * p.pooled;
-      const long bin = (long)n * PP + k;
-      Geom g;
-      deform_geom(p, n, 0, ph, pw, g);
-      AxisTab ax, ay;
-      axis_build(ax, g.wstart, g.sub_w, S, p.width);
-      axis_build(ay, g.hstart, g.sub_h, S, p.height);
-      const int cnt = ax.nvalid * ay.nvalid;
-      const float fc = (float)cnt;
-      if (!BWD) {
-        float sum[kTileCh];
-#pragma unroll
-        for (int c = 0; c < kTileCh; ++c) sum[c] = 0.f;
-        if (cnt) {
-          for (int a = 0; a < ay.n; ++a)
-            for (int e = 0; e < ax.n; ++e) {
-              const float wgt = ay.w[a] * ax.w[e];
-              if (wgt == 0.f) continue;
-              const float* t = tile + (ay.idx[a] * p.width + ax.idx[e]) * kTilePad;
-#pragma unroll
-              for (int c = 0; c < kTileCh; ++c) sum[c] = fmaf(wgt, t[c], sum[c]);
-            }
-        }
-        const float inv = cnt ? 1.0f / fc : 0.f;
-        float* o = p.top_data + bin * C + c0;
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<float4*>(o + q * 4) =
-              make_float4(sum[q * 4] * inv, sum[q * 4 + 1] * inv, sum[q * 4 + 2] * inv, sum[q * 4 + 3] * inv);
-        if (p.top_count) {
-          float* oc = p.top_count + bin * C + c0;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) *reinterpret_cast<float4*>(oc + q * 4) = make_float4(fc, fc, fc, fc);
-        }
-      } else {
-        float tdx = 0.f, tdy = 0.f;
-        if (cnt) {
-          float dv[kTileCh];
-          const float* td = p.top_diff + bin * C + c0;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(td) + q);
-            dv[q * 4] = __fdiv_rn(t.x, fc); dv[q * 4 + 1] = __fdiv_rn(t.y, fc);
-            dv[q * 4 + 2] = __fdiv_rn(t.z, fc); dv[q * 4 + 3] = __fdiv_rn(t.w, fc);
-          }
-          const float* img = p.data + (size_t)b * HW * C + c0;
-          for (int a = 0; a < ay.n; ++a)
-            for (int e = 0; e < ax.n; ++e) {
-              const float wgt = ay.w[a] * ax.w[e];
-              const int px = ay.idx[a] * p.width + ax.idx[e];
-              if (wgt != 0.f) {
-                float* t = tile + px * kTilePad;
-#pragma unroll
-                for (int c = 0; c < kTileCh; ++c) atomicAdd(t + c, wgt * dv[c]);
-              }
-              if (!p.no_trans) {
-                float dot = 0.f;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float4 U = __ldg(reinterpret_cast<const float4*>(img + (size_t)px * C) + q);
-                  dot += U.x * dv[q * 4] + U.y * dv[q * 4 + 1] + U.z * dv[q * 4 + 2] + U.w * dv[q * 4 + 3];
-                }
-                tdx += ay.w[a] * ax.d[e] * dot;
-                tdy += ay.d[a] * ax.w[e] * dot;
-              }
-            }
-        }
-        if (!p.no_trans) {
-          float* tp = trans_part + ((size_t)slice * nbins + bin) * 2;
-          tp[0] = tdx * p.trans_std * g.roi_width;
-          tp[1] = tdy * p.trans_std * g.roi_height;
-        }
-      }
-    }
-  }
-  if (BWD) {
-    __syncthreads();
-    float* dd = p.data_diff + (size_t)b * HW * C + c0;
-    for (int i = threadIdx.x; i < HW * 4; i += blockDim.x) {
-      const int px = i >> 2, q = i & 3;
-      const float* t = tile + px * kTilePad + q * 4;
-      float4* dst = reinterpret_cast<float4*>(dd + (size_t)px * C) + q;
-      float4 v = *dst;                                           // data_diff is accumulated into (kAddTo)
-      v.x += t[0]; v.y += t[1]; v.z += t[2]; v.w += t[3];
-      *dst = v;
-    }
-  }
-}
-
-// trans_diff[(n, 0|1, part_h, part_w)] += sum over the channel slices of the partial (tdx, tdy) of bin (n, ph, pw)
-__global__ void __launch_bounds__(256) trans_reduce_kernel(PsArgs p, const float* __restrict__ trans_part, int slices,
-                                                           long nbins) {
-  const int PP = p.pooled * p.pooled;
-  for (long bin = (long)blockIdx.x * blockDim.x + threadIdx.x; bin < nbins; bin += (long)gridDim.x * blockDim.x) {
-    float sx = 0.f, sy = 0.f;
-    for (int s = 0; s < slices; ++s) {
-      const float2 v = *reinterpret_cast<const float2*>(trans_part + ((size_t)s * nbins + bin) * 2);
-      sx += v.x;
-      sy += v.y;
-    }
-    const int n = (int)(bin / PP), k = (int)(bin - (long)n * PP);
-    const int ph = k / p.pooled, pw = k - ph * p.pooled;
-    const int part_h = (int)floorf(__fmul_rn(__fdiv_rn((float)ph, (float)p.pooled), (float)p.part_size));
-    const int part_w = (int)floorf(__fmul_rn(__fdiv_rn((float)pw, (float)p.pooled), (float)p.part_size));
-    const size_t tb = (((size_t)n * 2) * p.part_size + part_h) * p.part_size + part_w;
-    if (sx != 0.f) atomicAdd(p.trans_diff + tb, sx);
-    if (sy != 0.f) atomicAdd(p.trans_diff + tb + (size_t)p.part_size * p.part_size, sy);
-  }
-}
-
-bool tiled_ok(const PsArgs& a, int batch) {
-  return fast_nhwc_ok(a) && batch > 0 && a.channels % kTileCh == 0 &&
-         (size_t)a.height * a.width * kTilePad * sizeof(float) <= 100 * 1024;   // two CTAs per SM
-}
-
-template <bool BWD>
-int launch_tiled(const PsArgs& a, int batch, float* trans_part, cudaStream_t st) {
-  const size_t smem = (size_t)a.height * a.width * kTilePad * sizeof(float);
-  static bool attr_done[2][64] = {{false}};
-  int dev = 0;
-  SN_CUDA(cudaGetDevice(&dev));
-  if (dev >= 0 && dev < 64 && !attr_done[BWD ? 1 : 0][dev]) {
-    SN_CUDA(cudaFuncSetAttribute(deform_psroi_tiled_kernel<BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    attr_done[BWD ? 1 : 0][dev] = true;
-  }
-  deform_psroi_tiled_kernel<BWD><<<dim3(a.channels / kTileCh, batch, 1), 256, smem, st>>>(a, trans_part);
-  SN_LAUNCH_CHECK();
-  return 0;
-}
-
 int fill_common(PsArgs& a, const float* data, const float* rois, const float* trans, int num_rois, int channels,
                 int height, int width, float spatial_scale, int output_dim, int group_size, int pooled_size,
                 int part_size, int sample_per_part, float trans_std, int no_trans, int num_classes, int layout) {
@@ -852,62 +675,6 @@ int sniper_deform_psroi_bwd_fp64acc(const float* top_diff, const float* data, co
     ps_add_f64_kernel<<<(int)((trans_elems + 255) / 256), 256, 0, (cudaStream_t)stream>>>(trans_diff, acc + data_elems,
                                                                                            trans_elems);
   SN_LAUNCH_CHECK();
-  return 0;
-}
-
-// Chip-tiled variants of the two calls above for NHWC data with group_size 1 (the layout this framework runs): `batch`
-// = number of chips in `data` (ROI batch indices must lie in [0, batch)).  Return -2 (and set the error string) when
-// the shape does not qualify (H*W too large for the shared-memory tile, channels not a multiple of 16, ...): the
-// caller then uses the generic entry point.  Forward results equal sniper_deform_psroi_fwd bit for bit.
-int sniper_deform_psroi_fwd_tiled(const float* data, const float* rois, const float* trans, int num_rois, int batch,
-                                  int channels, int height, int width, float spatial_scale, int output_dim,
-                                  int group_size, int pooled_size, int part_size, int sample_per_part, float trans_std,
-                                  int no_trans, int num_classes, float* top_data, float* top_count, void* stream) {
-  PsArgs a;
-  if (fill_common(a, data, rois, trans, num_rois, channels, height, width, spatial_scale, output_dim, group_size,
-                  pooled_size, part_size, sample_per_part, trans_std, no_trans, num_classes, 1))
-    return -1;
-  a.top_data = top_data; a.top_count = top_count;
-  if (!tiled_ok(a, batch) || ((uintptr_t)top_data & 15) != 0 || (top_count && ((uintptr_t)top_count & 15) != 0)) {
-    sn::set_error("deform_psroi_fwd_tiled: shape / alignment not supported by the tiled kernel");
-    return -2;
-  }
-  if (num_rois == 0) return 0;
-  return launch_tiled<false>(a, batch, nullptr, (cudaStream_t)stream);
-}
-
-// bytes of scratch sniper_deform_psroi_bwd_tiled needs (0 when no_trans): one (tdx, tdy) pair per bin and channel slice
-size_t sniper_deform_psroi_bwd_tiled_workspace_bytes(int num_rois, int channels, int pooled_size, int no_trans) {
-  if (no_trans) return 0;
-  return (size_t)(channels / kTileCh) * num_rois * pooled_size * pooled_size * 2 * sizeof(float);
-}
-
-int sniper_deform_psroi_bwd_tiled(const float* top_diff, const float* data, const float* rois, const float* trans,
-                                  int num_rois, int batch, int channels, int height, int width, float spatial_scale,
-                                  int output_dim, int group_size, int pooled_size, int part_size, int sample_per_part,
-                                  float trans_std, int no_trans, int num_classes, float* data_diff, float* trans_diff,
-                                  void* workspace, size_t workspace_bytes, void* stream) {
-  PsArgs a;
-  if (fill_common(a, data, rois, trans, num_rois, channels, height, width, spatial_scale, output_dim, group_size,
-                  pooled_size, part_size, sample_per_part, trans_std, no_trans, num_classes, 1))
-    return -1;
-  SN_CHECK(no_trans || trans_diff != nullptr, "deformable psroi bwd: trans_diff is null");
-  a.top_diff = top_diff; a.data_diff = data_diff; a.trans_diff = trans_diff;
-  const size_t need = sniper_deform_psroi_bwd_tiled_workspace_bytes(num_rois, channels, pooled_size, no_trans);
-  if (!tiled_ok(a, batch) || ((uintptr_t)data_diff & 15) != 0 || ((uintptr_t)top_diff & 15) != 0) {
-    sn::set_error("deform_psroi_bwd_tiled: shape / alignment not supported by the tiled kernel");
-    return -2;
-  }
-  SN_CHECK(need == 0 || (workspace != nullptr && workspace_bytes >= need && ((uintptr_t)workspace & 7) == 0),
-           "deform_psroi_bwd_tiled: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
-  if (num_rois == 0) return 0;
-  if (launch_tiled<true>(a, batch, static_cast<float*>(workspace), (cudaStream_t)stream)) return -1;
-  if (!no_trans) {
-    const long nbins = (long)num_rois * pooled_size * pooled_size;
-    trans_reduce_kernel<<<(int)((nbins + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        a, static_cast<const float*>(workspace), channels / kTileCh, nbins);
-    SN_LAUNCH_CHECK();
-  }
   return 0;
 }
 

@@ -11,7 +11,6 @@ graph.  Frozen layers (conv0, bn0, stage1 -- FIXED_PARAMS, sniper_res101_e2e.yml
 forward only.
 """
 import math
-import os
 
 import numpy as np
 import torch
@@ -50,14 +49,9 @@ class Cfg:
     # fp16 between the two Casts, resnet_mx_101_e2e.py:405-406 and :250-252), BatchNorm arithmetic and statistics stay
     # fp32, the RPN / R-FCN heads stay fp32 (TF32 math) exactly where the reference keeps them fp32, and the optimizer
     # keeps fp32 master weights + momentum and rewrites the bf16 copies every step (multi_precision SGD).
-    bf16 = os.environ.get("SNIPER_BF16", "0") == "1"
+    bf16 = False
     wgrad_splits = 0                  # 0 = choose per layer (fill one wave of persistent CTAs)
-    # BN statistics accumulated by the producing conv's epilogue (per-warp column sums reduced in a fixed order +
-    # double REDs) instead of a separate colsum pass: one pass over the activation less per BatchNorm, so ON by default
-    # (SNIPER_FUSE_BN=0 restores the separate pass for A/B runs).
-    fuse_bn_stats = os.environ.get("SNIPER_FUSE_BN", "1") == "1"
-    # run weight gradients on a second stream (see WgradScheduler); SNIPER_WGRAD_STREAM=0/1 overrides for A/B runs
-    wgrad_stream = os.environ.get("SNIPER_WGRAD_STREAM", "1") == "1"
+    wgrad_stream = True               # run weight gradients on a second stream (see WgradScheduler)
     # TRAIN.AUTO_FOCUS (configs/faster/sniper_res101_e2e_autofocus.yml): train the FocusPixel branch conv_new_2/3/out
     # against the batch's `scale_label` (resnet_mx_101_e2e.py:259-267, 313-315)
     autofocus = False
@@ -339,27 +333,19 @@ class BN:
                 self.st.gamma.fill_(1.0)
 
     def fwd(self, x, cfg, relu=True, have_stats=False):
-        """have_stats: the producer of x already accumulated sum / sum-of-squares into self.st.sums."""
+        """have_stats: the producer of x already accumulated sum / sum-of-squares into self.st.sums_f; the finalisation
+        then rides in the apply kernel (sums_f is cleared by the end-of-step bn_param_grad_batched launch)."""
         if self.frozen:
             return ops.affine_act(x, self.st.scale, self.st.shift, relu=relu)
-        if have_stats and self.fused_apply:
-            return ops.bn_apply_train(x, self.st, eps=cfg.bn_eps, momentum=cfg.bn_momentum, relu=relu)
         if have_stats:
-            ops.bn_finalize(self.st, x.numel() // self.C, eps=cfg.bn_eps, momentum=cfg.bn_momentum)
-        else:
-            ops.bn_stats(x, self.st, eps=cfg.bn_eps, momentum=cfg.bn_momentum)
+            return ops.bn_apply_train(x, self.st, eps=cfg.bn_eps, momentum=cfg.bn_momentum, relu=relu)
+        ops.bn_stats(x, self.st, eps=cfg.bn_eps, momentum=cfg.bn_momentum)
         return ops.affine_act(x, self.st.scale, self.st.shift, relu=relu)
 
-    fuse = False   # set from Cfg.fuse_bn_stats by SniperResNet101
-
-    fused_apply = False   # set per instance by SniperResNet101: statistics go to st.sums_f and the finalisation rides in
-                          # the apply kernel (sums_f is cleared by the end-of-step bn_param_grad_batched launch)
-
     def stats_sink(self):
-        """The scratch a producer may accumulate this BN's input statistics into (None: compute them here)."""
-        if self.frozen or not BN.fuse:
-            return None
-        return self.st.sums_f if self.fused_apply else self.st.sums
+        """The scratch a producer accumulates this BN's input statistics into (per-warp column sums reduced in a fixed
+        order + double REDs in the conv epilogue: one pass over the activation less); None for a frozen BN."""
+        return None if self.frozen else self.st.sums_f
 
     defer = False   # set per instance by SniperResNet101: dgamma/dbeta of all layers by one bn_param_grad_batched launch
 
@@ -413,10 +399,9 @@ class Unit:
             a3 = self.conv2.fwd(a2, scale=self.bn3.st.scale, shift=self.bn3.st.shift, relu=True)
             res = x if self.dim_match else self.sc.fwd(a1)
             return self.conv3.fwd(a3, out=out, residual=res, stats=sink)
-        fused = BN.fuse
-        a1 = self.bn1.fwd(x, cfg, have_stats=x_has_stats and fused)
+        a1 = self.bn1.fwd(x, cfg, have_stats=x_has_stats)
         c1 = self.conv1.fwd(a1, stats=self.bn2.stats_sink())
-        a2 = self.bn2.fwd(c1, cfg, have_stats=fused)
+        a2 = self.bn2.fwd(c1, cfg, have_stats=True)
         if self.deform:
             off = self.offset.fwd(a2, out_dtype=torch.float32)                 # [N,H,W,96] fp32, 72 used
             col = ops.deform_im2col(a2, off, kh=3, kw=3, stride=1, dil=2, pad=2, dgroups=4)
@@ -425,7 +410,7 @@ class Unit:
         else:
             off = col = None
             c2 = self.conv2.fwd(a2, stats=self.bn3.stats_sink())
-        a3 = self.bn3.fwd(c2, cfg, have_stats=fused)
+        a3 = self.bn3.fwd(c2, cfg, have_stats=True)
         res = x if self.dim_match else self.sc.fwd(a1)
         y = self.conv3.fwd(a3, out=out, residual=res, stats=sink)
         self.saved = (x, a1, c1, a2, c2, a3, off, col)
@@ -497,7 +482,6 @@ class SniperResNet101:
         self.cfg = cfg or Cfg()
         cfg = self.cfg
         self.device = device
-        BN.fuse = bool(cfg.fuse_bn_stats)
         cfg.wsched = WgradScheduler(bool(cfg.wgrad_stream))
         self._wt_table = None
         self._bn_table = None
@@ -545,8 +529,6 @@ class SniperResNet101:
         P.finalize(device, lowp=bool(cfg.bf16))
         self.act_dtype = torch.bfloat16 if cfg.bf16 else torch.float32
         self._init_weights(seed, deform_offset_std)
-        for b in self.train_bns():
-            b.fused_apply = bool(cfg.fuse_bn_stats) and os.environ.get("SNIPER_BN_APPLY_FUSED", "1") == "1"
         # losses: [0:4] rpn_cls, rpn_bbox, rcnn_cls, rcnn_bbox sums; AutoFocus: [4] cls_scale_prob loss sum, [5:7] argmax
         # hits / non-ignored FocusPixels (exact float counts)
         self.loss_buf = torch.zeros(8, device=device)
@@ -938,11 +920,8 @@ class SniperResNet101:
         return [self.bn_data, self.bn0] + [b for u in self.units for b in u.bns()]
 
     def stem(self, data):
-        """bn_data -> conv0 -> bn0 -> ReLU (resnetc4 :402-408), NHWC out.  Default: im2col + wgmma GEMM (TF32 for the
-        fp32 configuration, bf16 operands in the mixed-precision one); SNIPER_STEM_TC=0: the FP32-FMA direct kernel."""
-        if os.environ.get("SNIPER_STEM_TC", "1") != "1":
-            return ops.stem_conv(data, self.conv0_w, self.bn_data.st.scale, self.bn_data.st.shift, self.bn0.st.scale,
-                                 self.bn0.st.shift, out_dtype=self.act_dtype)
+        """bn_data -> conv0 -> bn0 -> ReLU (resnetc4 :402-408), NHWC out: im2col + wgmma GEMM (TF32 for the fp32
+        configuration, bf16 operands in the mixed-precision one)."""
         if self._stem_rows is None:            # frozen layer: built once (load_reference resets it)
             self._stem_rows = ops.stem_rows(self.conv0_w, self.act_dtype)
         return ops.stem_conv_tc(data, self._stem_rows, self.bn_data.st.scale, self.bn_data.st.shift, self.bn0.st.scale,

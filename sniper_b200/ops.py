@@ -154,7 +154,7 @@ def deform_psroi_fwd(data, rois, trans, *, spatial_scale, output_dim, group_size
                      want_sample_idx=False):
     """DeformablePSROIPooling forward (deformable_psroi_pooling.cu:71-161)."""
     _f32(data), _f32(rois)
-    B, C, H, W = _ps_dims(data, layout)
+    _, C, H, W = _ps_dims(data, layout)
     N = rois.shape[0]
     P = pooled_size
     shape = (N, output_dim, P, P) if layout == NCHW else (N, P, P, output_dim)
@@ -163,30 +163,11 @@ def deform_psroi_fwd(data, rois, trans, *, spatial_scale, output_dim, group_size
     S = sample_per_part
     sidx = torch.empty(N * output_dim * P * P, S * S, 4, dtype=torch.int32, device=data.device) if want_sample_idx else None
     ncls = 1 if no_trans else trans.shape[1] // 2
-    if _psroi_tiled(layout, group_size, ncls, C, H, W, S) and not want_sample_idx:
-        rc = lib().sniper_deform_psroi_fwd_tiled(_ptr(data), _ptr(rois), _ptr(None if no_trans else _f32(trans)), N, B, C,
-                                                 H, W, float(spatial_scale), output_dim, group_size, P, part_size, S,
-                                                 float(trans_std), int(no_trans), ncls, _ptr(out), _ptr(cnt), _stream())
-        if rc != -2:
-            check(rc)
-            return out, cnt, sidx
     check(lib().sniper_deform_psroi_fwd(_ptr(data), _ptr(rois), _ptr(None if no_trans else _f32(trans)), N, C, H, W,
                                         float(spatial_scale), output_dim, group_size, P, part_size, S,
                                         float(trans_std), int(no_trans), ncls, layout, _ptr(out), _ptr(cnt),
                                         _ptr(sidx), _stream()))
     return out, cnt, sidx
-
-
-_psroi_ws = {}
-
-
-def _psroi_tiled(layout, group_size, ncls, C, H, W, S):
-    """True when the chip-tiled PSROI kernels are requested (SNIPER_PSROI_TILED=1) and apply; the library re-checks and
-    answers -2 otherwise.  Opt-in (not measured on the H100): with one lane per bin the shared-memory accesses of a warp
-    scatter over pixels (bank conflicts, CAS-loop float atomics), which can cost more than the global gathers / REDs it
-    removes."""
-    return (layout == NHWC and group_size == 1 and ncls == 1 and C % 16 == 0 and H * W * 17 * 4 <= 100 * 1024 and S <= 4
-            and os.environ.get("SNIPER_PSROI_TILED", "0") == "1" and os.environ.get("SNIPER_PSROI_EXACT") != "1")
 
 
 def deform_psroi_bwd(top_diff, data, rois, trans, *, spatial_scale, output_dim, group_size, pooled_size,
@@ -201,24 +182,6 @@ def deform_psroi_bwd(top_diff, data, rois, trans, *, spatial_scale, output_dim, 
     if trans_diff is None and not no_trans:
         trans_diff = torch.zeros_like(trans)
     ncls = 1 if no_trans else trans.shape[1] // 2
-    if _psroi_tiled(layout, group_size, ncls, C, H, W, sample_per_part):
-        need = int(lib().sniper_deform_psroi_bwd_tiled_workspace_bytes(N, C, pooled_size, int(no_trans)))
-        ws = None
-        if need:      # caller-owned scratch, kept per device and grown on demand (allocated outside any graph capture
-            key = (data.device.index, "psroi_bwd")      # by the first eager step; the captured steps reuse it)
-            ws = _psroi_ws.get(key)
-            if ws is None or ws.numel() < need:
-                ws = _psroi_ws[key] = torch.empty(need, dtype=torch.uint8, device=data.device)
-        rc = lib().sniper_deform_psroi_bwd_tiled(_ptr(top_diff), _ptr(data), _ptr(rois), _ptr(None if no_trans else trans),
-                                                 N, B, C, H, W, float(spatial_scale), output_dim, group_size, pooled_size,
-                                                 part_size, sample_per_part, float(trans_std), int(no_trans), ncls,
-                                                 _ptr(data_diff), _ptr(trans_diff), _ptr(ws), 0 if ws is None else ws.numel(),
-                                                 _stream())
-        if rc != -2:
-            check(rc)
-            if not no_trans:
-                _libmod.launches[0] += 1          # + trans_reduce_kernel (the counting proxy adds one per call)
-            return data_diff, trans_diff
     # product path (NHWC, one class, the channel counts of the warp-per-bin kernels, 16-byte aligned buffers): the
     # scattered contributions are summed in an fp64 scratch, which makes the gradients reproducible run to run
     if (layout == NHWC and group_size == 1 and ncls == 1 and sample_per_part <= 4 and C in (128, 256, 512)

@@ -24,7 +24,6 @@ class Trainer:
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
         self.world_size = world_size
-        self.overlap_allreduce = True     # False: one all-reduce of the whole buffer after the backward pass (A/B runs)
         self._works = []
         self.net = net if net is not None else model.SniperResNet101(self.cfg, device=self.device, seed=seed,
                                                                      deform_offset_std=deform_offset_std)
@@ -42,8 +41,6 @@ class Trainer:
         self.stage_free = [None, None]       # event: the step that consumed stage[i] has copied it out
         self.stage_owner = [None, None]      # the host batch object sitting in stage[i] (kept alive: identity match)
         self.next_stage = 0
-        import os
-        self.overlap_allreduce = os.environ.get("SNIPER_AR_OVERLAP", "1") == "1"
         # optimizer state of mxnet.optimizer.SGD that lives on the host: update count and LR schedule
         self.num_update = 0
         if scheduler == "config":
@@ -118,19 +115,15 @@ class Trainer:
         """Starts the sum of gradient bucket k over the ranks on NCCL's own stream (it first waits for everything
         enqueued so far on the current stream, i.e. the phase that produced the bucket) and returns at once, so the next
         backward phase overlaps the transfer.  No 1/N: rescale_grad = 1.0 (lib/train_utils/utils.py:30,37)."""
-        if self.world_size > 1 and self.overlap_allreduce:
+        if self.world_size > 1:
             a, b = self.net.P.bucket_ranges[k]
             self._works.append(torch.distributed.all_reduce(self.net.P.g[a:b], op=torch.distributed.ReduceOp.SUM,
                                                             async_op=True))
 
     def _allreduce_finish(self):
-        if self.world_size > 1:
-            if self.overlap_allreduce:
-                for w in self._works:
-                    w.wait()                      # the current stream waits for the collective
-                self._works = []
-            else:
-                self._allreduce()
+        for w in self._works:
+            w.wait()                              # the current stream waits for the collective
+        self._works = []
 
     def _snapshot(self):
         P = self.net.P

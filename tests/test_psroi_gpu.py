@@ -95,48 +95,6 @@ def test_deform_psroi_sniper_shape():
     np.testing.assert_allclose(g_td.cpu().numpy(), td, rtol=2e-3, atol=2e-3)
 
 
-@pytest.mark.parametrize("no_trans", [True, False])
-def test_deform_psroi_tiled_equals_warp_per_bin(no_trans):
-    """Chip-tiled kernels (one CTA per chip x 16 channels, shared-memory tile) vs the warp-per-bin kernels: forward
-    bit-identical (same per-channel operation order), backward equal up to the summation order of the scatter; ROIs of
-    the chips interleaved, one chip without ROIs, gradients accumulated into non-zero buffers (kAddTo)."""
-    import os
-    import torch
-    from sniper_b200 import ops
-    rng = np.random.RandomState(11)
-    B, C, N = 5, 256, 333
-    data = torch.from_numpy(rng.randn(B, 32, 32, C).astype(np.float32)).cuda()
-    rois = synth.rois_for_pool(rng, N, B)
-    rois[:, 0] = rng.permutation(N) % (B - 1)           # interleaved chips, chip B-1 gets no ROI
-    rois[::17, 1:] = [[-40, -30, 700, 560]]             # a few boxes larger than the chip: samples outside are skipped
-    rois = torch.from_numpy(rois).cuda()
-    trans = torch.from_numpy((rng.randn(N, 2, 7, 7) * 0.5).astype(np.float32)).cuda()
-    kw = dict(spatial_scale=0.0625, output_dim=C, group_size=1, pooled_size=7, part_size=7, sample_per_part=4,
-              trans_std=0.1, no_trans=no_trans, layout=1)
-    g = torch.from_numpy(rng.randn(N, 7, 7, C).astype(np.float32)).cuda()
-    dd0 = torch.from_numpy(rng.randn(B, 32, 32, C).astype(np.float32)).cuda()
-    td0 = torch.from_numpy(rng.randn(N, 2, 7, 7).astype(np.float32)).cuda()
-    res = {}
-    for tiled in ("1", "0"):
-        os.environ["SNIPER_PSROI_TILED"] = tiled
-        try:
-            ops.reset_launch_count()
-            out, cnt, _ = ops.deform_psroi_fwd(data, rois, trans, want_count=True, **kw)
-            dd, td = ops.deform_psroi_bwd(g, data, rois, trans, data_diff=dd0.clone(),
-                                          trans_diff=None if no_trans else td0.clone(), **kw)
-            res[tiled] = (out.cpu(), cnt.cpu(), dd.cpu(), None if no_trans else td.cpu())
-        finally:
-            os.environ.pop("SNIPER_PSROI_TILED", None)
-    a, b = res["1"], res["0"]
-    assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1])
-    scale = float((b[2] - dd0.cpu()).abs().max())
-    assert float((a[2] - b[2]).abs().max()) <= 2e-5 * scale
-    assert float((a[2][B - 1] - dd0.cpu()[B - 1]).abs().max()) == 0.0     # the chip without ROIs only keeps its old gradient
-    if not no_trans:
-        tscale = float((b[3] - td0.cpu()).abs().max())
-        assert float((a[3] - b[3]).abs().max()) <= 1e-4 * tscale
-
-
 @pytest.mark.parametrize("layout", [0, 1])
 def test_psroi(layout):
     from sniper_b200 import ops

@@ -1,5 +1,5 @@
 """Times the HBM-bound BatchNorm kernels alone (CUDA-graph replay of 20 launches over rotating buffers larger than L2)
-and prints algorithmic GB/s.  Usage: [GT_DTYPE=bf16] python tools/ew_time.py [ENV=VAL[,ENV=VAL] ...]"""
+and prints algorithmic GB/s.  Usage: [GT_DTYPE=bf16] python tools/ew_time.py"""
 import os
 import sys
 import torch
@@ -9,9 +9,6 @@ from sniper_b200 import ops
 DT = torch.bfloat16 if os.environ.get("GT_DTYPE") == "bf16" else torch.float32
 ES = 2 if DT == torch.bfloat16 else 4
 SHAPES = [(20480, 256), (20480, 1024), (81920, 128), (81920, 512), (327680, 64), (327680, 256)]
-SETTINGS = [{}]
-if len(sys.argv) > 1:
-    SETTINGS = [dict(kv.split("=") for kv in a.split(",") if kv) for a in sys.argv[1:]]
 
 
 def timed(fn, reps=20):
@@ -49,13 +46,6 @@ for M, C in SHAPES:
         "bwd+add(5r1w)": (lambda i: ops.bn_relu_bwd(X[i % nbuf], DY[i % nbuf], bn, add=DY[(i + 1) % nbuf], out=Y[i % nbuf]), 6),
     }
     for name, (fn, passes) in cases.items():
-        out = []
-        for stg in SETTINGS:
-            for k in ("SNIPER_EW_BPS", "SNIPER_EW_CLUSTER"):
-                os.environ.pop(k, None)
-            os.environ.update(stg)
-            us = timed(fn)
-            out.append("%s %.1f us %.2f TB/s" % (",".join("%s=%s" % kv for kv in stg.items()).replace("SNIPER_EW_", ""), us,
-                                                 passes * byts / us / 1e6))
-        print("%7d x %4d %-14s %s" % (M, C, name, " | ".join(out)), flush=True)
+        us = timed(fn)
+        print("%7d x %4d %-14s %.1f us %.2f TB/s" % (M, C, name, us, passes * byts / us / 1e6), flush=True)
     del X, DY, Y

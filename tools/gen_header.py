@@ -15,9 +15,6 @@ DOC = {
     "sniper_multi_proposal_workspace_bytes": "Scratch bytes for sniper_multi_proposal_fwd.",
     "sniper_multi_proposal_fwd": "Drop-in for the inference proposal operator MultiProposal (multi_proposal-inl.h:55-167: arguments cls_prob,bbox_pred,im_info -> outputs output(rois),score; CPU op multi_proposal.cc:273-374, GPU-build op multi_proposal.cu:400-631, which is host code with D2H copies). Decode + min-size filter + exact top-pre_nms_top_n selection + greedy NMS on device; flags 1 = the GPU build's anchor-type suppression. Rows after the kept ones: deterministic filler instead of the reference's rand() boxes.",
     "sniper_deform_psroi_fwd": "DeformablePSROIPoolingOp::Forward (contrib/deformable_psroi_pooling-inl.h:84-125, kernel .cu:71-161). top_count optional (hidden output of the reference), sample_idx optional parity output [count, spp^2, 4].",
-    "sniper_deform_psroi_fwd_tiled": "DeformablePSROIPoolingOp::Forward for NHWC data, group_size 1 (contrib/deformable_psroi_pooling-inl.h:84-125): chip-tiled kernel, one CTA per (chip, 16 channels) with the feature slice in shared memory; same results as sniper_deform_psroi_fwd. Returns -2 when the shape does not qualify.",
-    "sniper_deform_psroi_bwd_tiled_workspace_bytes": "Scratch bytes sniper_deform_psroi_bwd_tiled needs (the operator's kTempSpace request).",
-    "sniper_deform_psroi_bwd_tiled": "DeformablePSROIPoolingOp::Backward (-inl.h:127-174, kernel .cu:203-330) for NHWC data, group_size 1: gradient slice accumulated in shared memory (no global atomics), data_diff/trans_diff accumulated into (kAddTo). Returns -2 when the shape does not qualify.",
     "sniper_deform_psroi_bwd": "DeformablePSROIPoolingOp::Backward (contrib/deformable_psroi_pooling-inl.h:127-174, kernel .cu:203-330). data_diff/trans_diff are accumulated into (kAddTo); zero them for kWriteTo.",
     "sniper_deform_psroi_bwd_fp64acc": "sniper_deform_psroi_bwd on the NHWC kernels with the gradients summed in a caller-owned fp64 scratch (reproducible run to run); -2 if the shape does not qualify.",
     "sniper_psroi_fwd": "PSROIPoolingOp::Forward (contrib/psroi_pooling.cu:51-118). bins optional parity output [count,4] = hstart,hend,wstart,wend.",
