@@ -68,6 +68,7 @@ SIGNATURES = {
     "sniper_focus_label": ("i", "ppi" "iiii" "ddd" "pp"),
     "sniper_focus_acc": ("i", "pipl" "pp"),
     "sniper_soft_nms_batched": ("i", "ppifffuppp"),
+    "sniper_proposal_nms_batched": ("i", "pppippp"),
     "sniper_chip_input": ("i", "ppppiip"),
     "sniper_chip_input_hw": ("i", "ppppiiip"),
     "sniper_anchor_subsample": ("i", "pppiiiiiiup"),

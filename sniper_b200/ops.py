@@ -726,6 +726,27 @@ def soft_nms_batched(dets, offsets, *, sigma=0.55, Nt=0.3, threshold=0.001, meth
     return out, counts[:P]
 
 
+def proposal_nms_batched(dets, offsets):
+    """nmsp (lib/nms/nms.py:48-80, IoU threshold 0.7) of every image p = rows dets[offsets[p]:offsets[p+1]] at once.
+    dets: device float32 [total, 5] (x1, y1, x2, y2, score >= 0); offsets: host int32 [P+1], at most 4096 rows per
+    image.  Returns (keep, counts) on the host: keep[offsets[p]:offsets[p] + counts[p]] are image p's kept rows (indices
+    local to the image) in nmsp's keep order.  Waits for the launch."""
+    assert dets.is_cuda and dets.dtype == torch.float32 and dets.dim() == 2 and dets.shape[1] == 5 and dets.is_contiguous()
+    offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+    P = offsets.size - 1
+    assert P >= 0 and offsets[-1] == dets.shape[0]
+    off_dev = torch.from_numpy(offsets).to(dets.device)
+    counts = torch.zeros(max(P, 1), dtype=torch.int32, device=dets.device)
+    keep = torch.zeros(max(dets.shape[0], 1), dtype=torch.int32, device=dets.device)
+    check(lib().sniper_proposal_nms_batched(_ptr(dets), _ptr(off_dev), offsets.ctypes.data, P, _ptr(counts), _ptr(keep),
+                                            _stream()))
+    counts = counts[:P].cpu().numpy()
+    bad = np.where(counts < 0)[0]
+    if len(bad):
+        raise _libmod.SniperError("proposal_nms_batched: image %d has a negative score" % int(bad[0]))
+    return keep.cpu().numpy(), counts
+
+
 # ---------------------------------------------------------------------------------------------
 # MobileNetV2 layers (symbols/faster/mobilenetv2_e2e.py): depthwise 3x3, first-layer im2col, shortcut add
 # ---------------------------------------------------------------------------------------------

@@ -12,10 +12,17 @@ Host-side mirror of `lib/iterators/MNIteratorTestAutoFocus.py` (:13-141), `lib/i
   per-(image, class) cpu_soft_nms in a Pool(32)         ONE `sniper_soft_nms_batched` launch for the whole run
   FocusChips with OpenCV                                `chips_inference.add_chips`
 
+The proposal extraction of main_test.py with TEST.EXTRACT_PROPOSALS -- `MNIteratorTest`, `Tester.get_proposals` /
+`extract_proposals` and `imdb_proposal_extraction_wrapper` (lib/iterators/MNIteratorTest.py, lib/inference.py:76-98,
+372-409, 532-610) -- runs `SniperResNet101.forward_rpn` on whole images; `proposals.py` loads its output into the
+training roidb for negative-chip mining.
+
 roidb entries need `width`, `height`, `image_data` (decoded BGR uint8 [H,W,3]; this image has no OpenCV to decode files)
 or an `image_loader`; `inference_crops` is initialised to the full image like the reference does.
 """
 import math
+import os
+import pickle
 import time
 
 import numpy as np
@@ -25,7 +32,65 @@ from . import chips_inference, inference
 from ._lib import check, lib
 
 
-class MNIteratorTestAutoFocus(object):
+class _ImageCanvas(object):
+    """Pixel stage of the test iterators: uint8 source rectangles, resized by their scale and zero-padded into an
+    SH x SW canvas minus PIXEL_MEANS by one `sniper_chip_input_hw` launch per batch."""
+
+    def _init_canvas(self, config, device, image_loader):
+        self.device = torch.device(device)
+        self.image_loader = image_loader
+        self.on_gpu = self.device.type == "cuda"        # host-only use (tests of the batching logic): no canvas is built
+        self.means = torch.tensor(list(config.network.PIXEL_MEANS), dtype=torch.float32,
+                                  device=self.device if self.on_gpu else "cpu")
+        self._pix = None
+
+    def _image(self, r):
+        if 'image_data' in r:
+            return r['image_data']
+        if self.image_loader is None:
+            raise RuntimeError("roidb entry has no 'image_data' and no image_loader was given (no OpenCV in this image)")
+        return self.image_loader(r['image'])
+
+    def _canvas(self, rects, scales, SH, SW):
+        """rects: (image, y1, y2, x1, x2, flip) per batch entry.  Returns dict(data [n,3,SH,SW], im_info [n,3] =
+        (resized h, resized w, scale)) on the device, or the launch's inputs (pixels, table, canvas, im_info) on a
+        host-only iterator."""
+        n = len(rects)
+        need = sum(max(y2 - y1, 0) * max(x2 - x1, 0) * 3 for _, y1, y2, x1, x2, _ in rects)
+        pix = np.empty(need, dtype=np.uint8)
+        table = np.zeros((n, 8), dtype=np.int64)
+        im_info = np.zeros((n, 3), dtype=np.float32)
+        off = 0
+        for k, ((im, y1, y2, x1, x2, flip), scale) in enumerate(zip(rects, scales)):
+            h, w = max(y2 - y1, 0), max(x2 - x1, 0)
+            m = h * w * 3
+            if m:
+                pix[off:off + m].reshape(h, w, 3)[...] = im[y1:y2, x1:x2, :3]
+            dh, dw = int(np.rint(h * scale)), int(np.rint(w * scale))              # cv2.resize dsize = cvRound(...)
+            dh, dw = min(dh, SH), min(dw, SW)
+            table[k] = [off, h, w, dh, dw, 1 if flip else 0, int(np.float64(scale).view(np.int64)), 0]
+            im_info[k] = [dh, dw, scale]
+            off += m
+        if not self.on_gpu:
+            return dict(pixels=pix, table=table, canvas=(SH, SW), im_info=torch.from_numpy(im_info))
+        dev = self.device
+        if self._pix is None or self._pix.numel() < need:
+            self._pix = torch.empty(int(need * 1.25) + 4096, dtype=torch.uint8, device=dev)
+        self._pix[:need].copy_(torch.from_numpy(pix), non_blocking=True)
+        tab = torch.from_numpy(table).to(dev)
+        data = torch.empty(n, 3, SH, SW, device=dev)
+        check(lib().sniper_chip_input_hw(self._pix.data_ptr(), tab.data_ptr(), self.means.data_ptr(), data.data_ptr(), n, SH,
+                                         SW, torch.cuda.current_stream().cuda_stream))
+        return dict(data=data, im_info=torch.from_numpy(im_info).to(dev))
+
+
+def _canvas_size(h, w):
+    """The network needs a canvas that survives the stride-16 backbone; the conv kernel wants every layer's output width
+    to be a multiple of 8 pixels (stride 16 -> the canvas width a multiple of 128), heights are free (multiple of 32)."""
+    return -(-h // 32) * 32, -(-w // 128) * 128
+
+
+class MNIteratorTestAutoFocus(_ImageCanvas):
     """MNIteratorTestAutoFocus(roidb, config, test_scale, batch_size, ...): batches of chips of one test scale, sorted by
     area and grouped by orientation (reset :88-141); a batch is padded to its largest resized chip (_get_batch :36-78)."""
 
@@ -33,13 +98,8 @@ class MNIteratorTestAutoFocus(object):
                  num_classes=None, device="cuda:0", image_loader=None):
         self.roidb, self.cfg, self.test_scale = roidb, config, test_scale
         self.batch_size = batch_size
-        self.device = torch.device(device)
-        self.image_loader = image_loader
         self.data_name = ['data', 'im_info', 'im_ids', 'chip_ids']
-        self.on_gpu = self.device.type == "cuda"        # host-only use (tests of the batching logic): no canvas is built
-        self.means = torch.tensor(list(config.network.PIXEL_MEANS), dtype=torch.float32,
-                                  device=self.device if self.on_gpu else "cpu")
-        self._pix = None
+        self._init_canvas(config, device, image_loader)
         self.reset()
 
     def set_scale(self, scale):
@@ -88,13 +148,6 @@ class MNIteratorTestAutoFocus(object):
     def get_batch_size(self):
         return self.batch_size
 
-    def _image(self, r):
-        if 'image_data' in r:
-            return r['image_data']
-        if self.image_loader is None:
-            raise RuntimeError("roidb entry has no 'image_data' and no image_loader was given (no OpenCV in this image)")
-        return self.image_loader(r['image'])
-
     def __next__(self):
         if self.cur_i >= self.size:
             raise StopIteration
@@ -119,39 +172,72 @@ class MNIteratorTestAutoFocus(object):
             im = self._image(r)
             y1, y2 = max(int(cur_chip[1]), 0), min(int(cur_chip[3]), im.shape[0])     # worker_autofocus :60-62
             x1, x2 = max(int(cur_chip[0]), 0), min(int(cur_chip[2]), im.shape[1])
-            rects.append((im, y1, y2, x1, x2))
+            rects.append((im, y1, y2, x1, x2, False))
             scales.append(scale)
-        # the network needs a canvas that survives the stride-16 backbone; the conv kernel wants every layer's output width
-        # to be a multiple of 8 pixels (stride 16 -> the canvas width a multiple of 128), heights are free (multiple of 32)
-        SH, SW = -(-max_size[0] // 32) * 32, -(-max_size[1] // 128) * 128
-        need = sum(max(y2 - y1, 0) * max(x2 - x1, 0) * 3 for _, y1, y2, x1, x2 in rects)
-        pix = np.empty(need, dtype=np.uint8)
-        table = np.zeros((n, 8), dtype=np.int64)
-        im_info = np.zeros((n, 3), dtype=np.float32)
-        off = 0
-        for k, ((im, y1, y2, x1, x2), scale) in enumerate(zip(rects, scales)):
-            h, w = max(y2 - y1, 0), max(x2 - x1, 0)
-            m = h * w * 3
-            if m:
-                pix[off:off + m].reshape(h, w, 3)[...] = im[y1:y2, x1:x2, :3]
-            dh, dw = int(np.rint(h * scale)), int(np.rint(w * scale))              # cv2.resize dsize = cvRound(...)
-            dh, dw = min(dh, SH), min(dw, SW)
-            table[k] = [off, h, w, dh, dw, 0, int(np.float64(scale).view(np.int64)), 0]
-            im_info[k] = [dh, dw, scale]
-            off += m
-        if not self.on_gpu:
-            return dict(pixels=pix, table=table, canvas=(SH, SW), im_info=torch.from_numpy(im_info),
-                        im_ids=np.array(im_ids, dtype=int), chip_ids=local_chip_ids.astype(int), scales=np.array(scales))
-        dev = self.device
-        if self._pix is None or self._pix.numel() < need:
-            self._pix = torch.empty(int(need * 1.25) + 4096, dtype=torch.uint8, device=dev)
-        self._pix[:need].copy_(torch.from_numpy(pix), non_blocking=True)
-        tab = torch.from_numpy(table).to(dev)
-        data = torch.empty(n, 3, SH, SW, device=dev)
-        check(lib().sniper_chip_input_hw(self._pix.data_ptr(), tab.data_ptr(), self.means.data_ptr(), data.data_ptr(), n, SH,
-                                         SW, torch.cuda.current_stream().cuda_stream))
-        return dict(data=data, im_info=torch.from_numpy(im_info).to(dev), im_ids=np.array(im_ids, dtype=int),
-                    chip_ids=local_chip_ids.astype(int), scales=np.array(scales))
+        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1]))
+        out.update(im_ids=np.array(im_ids, dtype=int), chip_ids=local_chip_ids.astype(int), scales=np.array(scales))
+        return out
+
+
+class MNIteratorTest(_ImageCanvas):
+    """MNIteratorTest(roidb, config, test_scale, batch_size, ...) (lib/iterators/MNIteratorTest.py): batches of whole
+    images at one test scale, horizontal images first, then vertical ones (reset :50-66).  Each image is resized by
+    `chips_inference.image_scale`.  The canvas is the test scale (swapped for vertical images) rounded up to the conv
+    kernel's multiples, the same for every batch of an orientation, so an image's proposals do not depend on which
+    images share its batch.  (The score-0 filler rows MultiProposal appends when an image has fewer than 300 proposals
+    do: their boxes follow the image's position in the batch, as the reference's rand() boxes follow the call order.)"""
+
+    def __init__(self, roidb, config, test_scale, batch_size=4, threads=8, nGPUs=1, pad_rois_to=400, crop_size=None,
+                 num_classes=None, device="cuda:0", image_loader=None):
+        self.roidb, self.cfg, self.test_scale = roidb, config, test_scale
+        self.batch_size = batch_size
+        self.data_name = ['data', 'im_info', 'im_ids']
+        self._init_canvas(config, device, image_loader)
+        self.reset()
+
+    def set_scale(self, scale):
+        self.test_scale = scale
+
+    def reset(self):
+        """self.inds: image indices in batch order; a group that does not fill its last batch repeats its first image."""
+        self.cur_i = 0
+        widths = np.array([r['width'] for r in self.roidb])
+        heights = np.array([r['height'] for r in self.roidb])
+        bs = self.batch_size
+        groups = []
+        for g in (np.where(widths >= heights)[0], np.where(widths < heights)[0]):
+            if g.shape[0] % bs > 0:
+                g = np.hstack((g, g[np.zeros(bs - g.shape[0] % bs, dtype=int)]))
+            groups.append(g)
+        self.inds = np.hstack(groups).astype(int)
+        self.size = len(self.inds)
+
+    def __iter__(self):
+        return self
+
+    def get_batch_size(self):
+        return self.batch_size
+
+    def __next__(self):
+        if self.cur_i >= self.size:
+            raise StopIteration
+        im_ids = [int(self.inds[i % self.size]) for i in range(self.cur_i, self.cur_i + self.batch_size)]
+        self.cur_i += self.batch_size
+        return self._get_batch([self.roidb[i] for i in im_ids], im_ids)
+
+    next = __next__
+
+    def _get_batch(self, roidb, im_ids):
+        hor = roidb[0]['width'] >= roidb[0]['height']
+        max_size = (self.test_scale[0], self.test_scale[1]) if hor else (self.test_scale[1], self.test_scale[0])
+        rects, scales = [], []
+        for r in roidb:
+            im = self._image(r)
+            rects.append((im, 0, im.shape[0], 0, im.shape[1], bool(r.get('flipped', False))))
+            scales.append(chips_inference.image_scale(r['width'], r['height'], self.test_scale))
+        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1]))
+        out.update(im_ids=np.array(im_ids, dtype=int), scales=np.array(scales))
+        return out
 
 
 class Tester(object):
@@ -164,6 +250,34 @@ class Tester(object):
         self.num_images = len(roidb)
         self.num_classes = num_classes or (imdb.num_classes if imdb is not None else cfg.dataset.NUM_CLASSES)
         self.detect_time = self.post_time = 0.0
+
+    def get_proposals(self, batch, scales):
+        """(scores, rois, batch, im_ids) of one batch (:76-98) from `net.forward_rpn`: per image its rpn scores [R] and
+        boxes [R,4] in ORIGINAL-image scale (rois / float32 im_info scale)."""
+        rois, rscores = self.net.forward_rpn(batch['data'], batch['im_info'])
+        rois, rscores = rois.cpu().numpy(), rscores.cpu().numpy().reshape(-1)
+        scores, boxes = [], []
+        for idx in range(batch['data'].shape[0]):
+            cids = np.where(rois[:, 0] == idx)[0]
+            boxes.append(rois[cids, 1:] / np.float32(scales[idx]))
+            scores.append(rscores[cids])
+        return scores, boxes, batch, batch['im_ids']
+
+    def extract_proposals(self, n_proposals=300, cache_name='cache', vis=False, vis_ext='.png'):
+        """all_boxes[image] = float32 [n_proposals, 5] (x1, y1, x2, y2, score) (:372-409): every image's first
+        n_proposals rows, in original-image coordinates."""
+        all_boxes = [[] for _ in range(self.num_images)]
+        for batch in self.test_iter:
+            scales = batch['im_info'].cpu().numpy()[:, 2]
+            t0 = time.time()
+            scores, boxes, _, im_ids = self.get_proposals(batch, scales)
+            self.detect_time += time.time() - t0
+            t0 = time.time()
+            for cscores, cboxes, im_id in zip(scores, boxes, im_ids):
+                all_boxes[im_id] = np.hstack((cboxes[0:n_proposals, 0:4],
+                                              cscores[0:n_proposals, np.newaxis])).astype(np.float32)
+            self.post_time += time.time() - t0
+        return all_boxes
 
     def detect(self, batch, scales=None):
         """(scores, boxes, data, im_ids, maps, chip_ids) of one batch (:100-139): scores [R,K] and boxes [R,4] per chip,
@@ -248,3 +362,30 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     torch.cuda.synchronize()
     stats['nms_s'] = time.time() - t0
     return all_boxes, stats
+
+
+def proposal_file_name(config):
+    """`<DATASET>_<test_image_set>_rpn.pkl`, the name main_test.py gives the extracted proposals (lib/inference.py:606)."""
+    return '{}_{}_rpn.pkl'.format(config.dataset.dataset.upper(), config.dataset.test_image_set)
+
+
+def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0"):
+    """The CONCURRENT_JOBS == 1 path of imdb_proposal_extraction_wrapper (:559-610): RPN proposals of every image at every
+    scale of TEST.SCALES (`net.forward_rpn`), each image's rows stacked in scale order, pickled as a list of float32
+    [n, 5] arrays to save_path/proposal_file_name(config) (protocol 2, readable by the reference's Python 2).  Returns
+    (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds."""
+    T = config.TEST
+    proposals, stats = [], dict(scales=[])
+    nb = batch_images or list(T.BATCH_IMAGES)
+    for nbatch, scale in zip(nb, T.SCALES):
+        it = MNIteratorTest(roidb, config, scale, batch_size=nbatch, device=device)
+        tester = Tester(net, None, roidb, it, config, batch_size=nbatch, num_classes=1)
+        t0 = time.time()
+        proposals.append(tester.extract_proposals(n_proposals=n_proposals))
+        stats['scales'].append(dict(scale=tuple(scale), images=len(roidb), batches=int(it.size // max(nbatch, 1)),
+                                    detect_s=tester.detect_time, post_s=tester.post_time, total_s=time.time() - t0))
+    final = [np.vstack([p[i] for p in proposals]) for i in range(len(roidb))]
+    os.makedirs(save_path, exist_ok=True)
+    with open(os.path.join(save_path, proposal_file_name(config)), 'wb') as f:
+        pickle.dump(final, f, protocol=2)
+    return final, stats
