@@ -827,6 +827,7 @@ int sniper_gemm_nt(const void* A, long lda, const void* B, long ldb, float* C, l
   SN_CHECK(K % E == 0 && K > 0, "gemm: K (%d) must be a positive multiple of %d", K, E);
   SN_CHECK(M > 0 && N > 0, "gemm: empty problem");
   SN_CHECK((lda * esz) % 16 == 0 && (ldb * esz) % 16 == 0, "gemm: row strides must be 16-byte multiples");
+  SN_CHECK(!(accumulate && out_bf16), "gemm: accumulate needs an fp32 output (bf16 outputs are stored, not added to)");
   GemmParams p;
   memset(&p, 0, sizeof(p));
   const int bn = pick_block_n(N);
@@ -868,6 +869,7 @@ int sniper_conv2d_nhwc(const void* X, long x_ld, int NB, int H, int W, int Cin, 
   SN_CHECK(Cin % E == 0, "conv: Cin (%d) must be a multiple of %d", Cin, E);
   SN_CHECK(ntaps >= 1 && ntaps <= kMaxTaps, "conv: ntaps (%d) out of range", ntaps);
   SN_CHECK(stride == 1 || stride == 2, "conv: stride must be 1 or 2");
+  SN_CHECK(!(accumulate && out_bf16), "conv: accumulate needs an fp32 output (bf16 outputs are stored, not added to)");
   // 128 output pixels per tile as tile_h rows x tile_w columns, tile_w = the largest power of two <= 128 dividing Wo
   // (training shapes: Wo = 32 ... 128 -> whole rows; inference canvases of any width that is a multiple of 8 pixels at
   // this layer's stride: narrower, taller tiles; rows past Ho are zero-filled by the TMA and not stored)

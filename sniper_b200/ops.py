@@ -260,6 +260,9 @@ def gemm_nt(a, b, *, out=None, scale=None, bias=None, residual=None, relu=False,
     if out is None:
         out = torch.empty(M, N, device=a.device, dtype=out_dtype or a.dtype)
     out_bf16 = out.dtype == torch.bfloat16
+    assert out.shape == (M, N) and out.stride(1) == 1, "out must be [M, N] with unit column stride"
+    assert residual is None or (residual.shape == (M, N) and residual.stride(1) == 1), \
+        "residual must be [M, N] with unit column stride"
     assert residual is None or residual.dtype == out.dtype, "bf16 output takes a bf16 residual"
     check(lib().sniper_gemm_nt(_ptr(a), a.stride(0), _ptr(b), b.stride(0), _ptr(out), out.stride(0), M, N, K, _dt(a),
                                _ptr(scale), _ptr(bias), _ptr(residual), 0 if residual is None else residual.stride(0),
@@ -304,6 +307,16 @@ def conv2d_nhwc(x, w, *, kh, kw, stride=1, dil=1, pad=0, out=None, scale=None, b
     return out
 
 
+def _pixel_ld(t):
+    """Row stride (elements) of an NHWC tensor whose pixels are equally spaced rows of contiguous channels."""
+    assert t.dim() == 4 and t.stride(3) == 1
+    NB, H, W, _ = t.shape
+    ld = t.stride(2)
+    assert (H == 1 or t.stride(1) == W * ld) and (NB == 1 or t.stride(0) == H * W * ld), \
+        "NHWC pixel rows must be uniformly strided"
+    return ld
+
+
 def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, splits=8, taps=None):
     """dW[Cout, kh*kw*Cin] += dY^T * im2col(X).  dy: [N,Ho,Wo,Cout], x: [N,H,W,Cin]."""
     NB, H, W, Cin = x.shape
@@ -311,12 +324,15 @@ def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, spl
     dh, dw = taps if taps is not None else conv_taps(kh, kw, dil, pad)
     ntaps = len(dh)
     _ensure_gemm_workspace(x.device)
-    assert dy.dtype == x.dtype
+    assert dy.dtype == x.dtype and dy.shape[0] == NB
+    dy_ld, x_ld = _pixel_ld(dy), _pixel_ld(x)
     if dw_out is None:
         dw_out = torch.zeros(Cout, ntaps * Cin, device=x.device)
+    assert dw_out.dtype == torch.float32 and dw_out.is_contiguous() and dw_out.shape == (Cout, ntaps * Cin), \
+        "dw_out must be a contiguous fp32 [Cout, taps * Cin]"
     _, dhp = _iarr(dh)
     _, dwp = _iarr(dw)
-    check(lib().sniper_conv2d_wgrad_nhwc(_ptr(dy), dy.stride(2), _ptr(x), x.stride(2), NB, H, W, Cin, Cout, ntaps, dhp,
+    check(lib().sniper_conv2d_wgrad_nhwc(_ptr(dy), dy_ld, _ptr(x), x_ld, NB, H, W, Cin, Cout, ntaps, dhp,
                                          dwp, stride, Ho, Wo,
                                          _ptr(dw_out), _dt(x), splits, _stream()))
     return dw_out
@@ -588,6 +604,8 @@ def bn_param_grad_batched(table):
 
 def colsum_accum(x, out):
     M, C, ldx = _rows(x)
+    assert x.dtype == torch.float32 and out.dtype == torch.float32 and out.shape == (C,) and out.is_contiguous(), \
+        "column sums read an fp32 [M, C] and add to an fp32 [C]"
     check(lib().sniper_colsum(_ptr(x), ldx, M, C, _ptr(out), _stream()))
     return out
 

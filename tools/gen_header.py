@@ -19,7 +19,7 @@ DOC = {
     "sniper_deform_psroi_bwd_fp64acc": "sniper_deform_psroi_bwd on the NHWC kernels with the gradients summed in a caller-owned fp64 scratch (reproducible run to run); -2 if the shape does not qualify.",
     "sniper_psroi_fwd": "PSROIPoolingOp::Forward (contrib/psroi_pooling.cu:51-118). bins optional parity output [count,4] = hstart,hend,wstart,wend.",
     "sniper_psroi_bwd": "PSROIPoolingOp::Backward (contrib/psroi_pooling.cu:146-210); accumulates into data_diff.",
-    "sniper_gemm_nt": "C[M,N] = epi(A[M,K] * B[N,K]^T) on wgmma (register accumulators, TMA operands). Replaces FullyConnected -> cuBLAS (nn/fully_connected-inl.h) and linalg_gemm (contrib/deformable_convolution-inl.h:148-160). dtype 0 = fp32 storage / TF32 math, 1 = bf16. epi: *scale[n], +bias[n], +residual[m,n], relu; accumulate = red.global.add.",
+    "sniper_gemm_nt": "C[M,N] = epi(A[M,K] * B[N,K]^T) on wgmma (register accumulators, TMA operands). Replaces FullyConnected -> cuBLAS (nn/fully_connected-inl.h) and linalg_gemm (contrib/deformable_convolution-inl.h:148-160). dtype 0 = fp32 storage / TF32 math, 1 = bf16. epi: *scale[n], +bias[n], +residual[m,n], relu; accumulate = red.global.add (fp32 outputs only; refused with out_bf16).",
     "sniper_gemm_plan": "Host-only: the tile width, ring depth, persistent grid and tail split sniper_gemm_nt would choose for a shape (no GPU needed).",
     "sniper_gemm_tail_workspace_bytes": "Size of the caller-owned scratch the wgmma kernel's split-K weight gradient uses (per device).",
     "sniper_gemm_set_tail_workspace": "Registers that scratch (zero-filled, caller-owned, must outlive later launches); the library itself never allocates device memory.",
