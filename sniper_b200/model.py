@@ -394,11 +394,7 @@ class Unit:
         this unit's output (its statistics are accumulated by conv3's epilogue)."""
         sink = next_bn.stats_sink() if next_bn is not None else None
         if self.frozen:
-            a1 = self.bn1.fwd(x, cfg)
-            a2 = self.conv1.fwd(a1, scale=self.bn2.st.scale, shift=self.bn2.st.shift, relu=True)
-            a3 = self.conv2.fwd(a2, scale=self.bn3.st.scale, shift=self.bn3.st.shift, relu=True)
-            res = x if self.dim_match else self.sc.fwd(a1)
-            return self.conv3.fwd(a3, out=out, residual=res, stats=sink)
+            return self.fwd_infer(x, cfg, out=out, stats=sink)
         a1 = self.bn1.fwd(x, cfg, have_stats=x_has_stats)
         c1 = self.conv1.fwd(a1, stats=self.bn2.stats_sink())
         a2 = self.bn2.fwd(c1, cfg, have_stats=True)
@@ -416,9 +412,10 @@ class Unit:
         self.saved = (x, a1, c1, a2, c2, a3, off, col)
         return y
 
-    def fwd_infer(self, x, cfg, out=None):
+    def fwd_infer(self, x, cfg, out=None, stats=None):
         """Inference forward (is_train=False: every BatchNorm uses its moving statistics, resnet_mx_101_e2e.py:36-69 with
-        use_global_stats): BN + ReLU ride in the producing conv's epilogue as per-channel scale/shift."""
+        use_global_stats): BN + ReLU ride in the producing conv's epilogue as per-channel scale/shift.  Also the
+        training forward of a frozen unit; `stats` then receives the next BatchNorm's input statistics from conv3."""
         a1 = ops.affine_act(x, self.bn1.st.scale, self.bn1.st.shift, relu=True)
         a2 = self.conv1.fwd(a1, scale=self.bn2.st.scale, shift=self.bn2.st.shift, relu=True)
         if self.deform:
@@ -429,7 +426,7 @@ class Unit:
         else:
             a3 = self.conv2.fwd(a2, scale=self.bn3.st.scale, shift=self.bn3.st.shift, relu=True)
         res = x if self.dim_match else self.sc.fwd(a1)
-        return self.conv3.fwd(a3, out=out, residual=res)
+        return self.conv3.fwd(a3, out=out, residual=res, stats=stats)
 
     def bwd(self, dout, cfg, extra_add=None):
         """dout: grad of the unit output [N,Ho,Wo,cout] (may be a channel slice).  Returns grad of the input
@@ -475,6 +472,105 @@ class Unit:
 
 
 # ------------------------------------------------------------------------------------------------
+# RPN / R-FCN head steps of SniperResNet101 and model_mnv2.SniperMobileNetV2, reading only what both nets hold under the
+# same names (cfg, rpn_conv, rpn_head, conv_new_1, fc_offset, fc_new_1, fc_new_2, fc_out, loss_buf, cnt_buf).  The
+# R-FCN losses stay with each net: their normalisations differ.
+def rpn_train(net, batch, head):
+    """RPN losses into loss_buf[0:2] and MultiProposalTarget on the device (resnet_mx_101_e2e.py:279-284).  head:
+    rpn_head's output, 4A deltas | 2A scores.  Returns (prob, dhead, rois, label, bbox_target, bbox_weight)."""
+    cfg = net.cfg
+    A = cfg.num_anchors
+    dhead = torch.zeros_like(head)
+    prob = torch.empty(*head.shape[:3], 2 * A, device=head.device)
+    ops.count_valid(batch["label"], net.cnt_buf[0:1])
+    ops.rpn_softmax_loss(head[..., 4 * A:6 * A], batch["label"], A, cfg.grad_scale, net.cnt_buf[0:1], prob,
+                         dhead[..., 4 * A:6 * A], net.loss_buf[0:1])
+    ops.rpn_smooth_l1_loss(head, batch["bbox_target"], batch["bbox_weight"], 4 * A,
+                           3.0 * cfg.grad_scale / float(cfg.batch_images * cfg.rpn_batch_size), dhead,
+                           net.loss_buf[1:2])
+    rois, label, bbox_target, bbox_weight = ops.multi_proposal_target(
+        prob, head, batch["im_info"], batch["gt_boxes"], batch["valid_ranges"], feat_stride=cfg.feat_stride,
+        scales=cfg.scales, ratios=cfg.ratios, rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, layout=ops.NHWC)
+    return prob, dhead, rois, label, bbox_target, bbox_weight
+
+
+def rpn_proposals(net, head, im_info, **kw):
+    """SoftmaxActivation over the RPN scores (rpn_softmax_loss with every label ignored) -> MultiProposal
+    (resnet_mx_101_e2e.py:342-355); kw: more ops.multi_proposal arguments.  Returns rois [B*R,5], scores [B*R] and the
+    softmax's (count, loss) scratch for rfcn_detect's class softmax."""
+    cfg = net.cfg
+    A = cfg.num_anchors
+    B, Hf, Wf = head.shape[:3]
+    dev = head.device
+    prob = torch.empty(B, Hf, Wf, 2 * A, device=dev)
+    ignore = torch.full((B, A * Hf * Wf), -1.0, device=dev)
+    cnt = torch.ones(1, dtype=torch.int32, device=dev)
+    loss = torch.zeros(1, device=dev)
+    ops.rpn_softmax_loss(head[..., 4 * A:6 * A], ignore, A, 1.0, cnt, prob, None, loss)
+    rois, scores = ops.multi_proposal(prob, head, im_info, feat_stride=cfg.feat_stride, scales=cfg.scales,
+                                      ratios=cfg.ratios, rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, layout=ops.NHWC,
+                                      **kw)
+    return rois, scores, cnt, loss
+
+
+def rfcn_fwd(net, feat, rois):
+    """Deformable R-FCN head (resnet_mx_101_e2e.py:286-303, 357-379) on conv_new_1's output: returns the fused
+    cls_score | bbox_pred FC output [N, fc_out.coutp] and the tensors head_bwd reads."""
+    N = rois.shape[0]
+    ps = dict(spatial_scale=1.0 / net.cfg.feat_stride, output_dim=256, group_size=1, pooled_size=7, part_size=7,
+              sample_per_part=4, layout=ops.NHWC)
+    offset_t, _, _ = ops.deform_psroi_fwd(feat, rois, None, no_trans=True, want_count=False, **ps)
+    off = ops.gemm_nt(offset_t.view(N, -1), net.fc_offset.w, bias=net.fc_offset.b)          # [N,128], 98 used
+    trans = off[:, :98].contiguous().view(N, 2, 7, 7)
+    pooled, _, _ = ops.deform_psroi_fwd(feat, rois, trans, no_trans=False, trans_std=0.1, want_count=False, **ps)
+    fc1 = ops.gemm_nt(pooled.view(N, -1), net.fc_new_1.w, bias=net.fc_new_1.b, relu=True)
+    fc2 = ops.gemm_nt(fc1, net.fc_new_2.w, bias=net.fc_new_2.b, relu=True)
+    out = ops.gemm_nt(fc2, net.fc_out.w, bias=net.fc_out.b)
+    return out, (ps, feat, rois, offset_t, off, trans, pooled, fc1, fc2)
+
+
+def rfcn_detect(net, head, feat, im_info, **kw):
+    """The inference tail: rpn_proposals -> rfcn_fwd -> SoftmaxActivation over the class scores (:380) ->
+    (rois [B*R,5], rpn scores [B*R], cls_prob [B*R,K], bbox_pred [B*R,4])."""
+    rois, scores, cnt, loss = rpn_proposals(net, head, im_info, **kw)
+    out, _ = rfcn_fwd(net, feat, rois)
+    N, K = rois.shape[0], net.cfg.num_classes
+    cls_prob = torch.empty(N, K, device=out.device)
+    lab = torch.full((N,), -1.0, device=out.device)
+    ops.softmax_ce(out, lab, K, 1.0, cnt, cls_prob, None, loss)
+    return rois, scores, cls_prob, out[:, K:K + 4]
+
+
+def head_bwd(net, x, rpn, dhead, dout, saved):
+    """Backward of both heads from dout (R-FCN) and dhead (RPN) to the fp32 gradient of their input x; rpn: rpn_conv's
+    output, saved: from rfcn_fwd.  Weight gradients go through cfg.wsched."""
+    sp, W = net.cfg.wgrad_splits, net.cfg.wsched
+    ps, feat, rois, offset_t, off, trans, pooled, fc1, fc2 = saved
+    N = rois.shape[0]
+    v4 = lambda t: t.view(1, 1, t.shape[0], t.shape[1])
+    W(net.fc_out.bwd_weight, v4(dout), v4(fc2), sp)
+    dfc2 = ops.relu_bwd(fc2, ops.gemm_nt(dout, net.fc_out.wt))
+    W(net.fc_new_2.bwd_weight, v4(dfc2), v4(fc1), sp)
+    dfc1 = ops.relu_bwd(fc1, ops.gemm_nt(dfc2, net.fc_new_2.wt))
+    W(net.fc_new_1.bwd_weight, v4(dfc1), v4(pooled.view(N, -1)), sp)
+    dpooled = ops.gemm_nt(dfc1, net.fc_new_1.wt).view(pooled.shape)
+    dfeat, dtrans = ops.deform_psroi_bwd(dpooled, feat, rois, trans, no_trans=False, trans_std=0.1, **ps)
+    doff = torch.zeros_like(off)
+    doff[:, :98] = dtrans.view(N, 98)
+    W(net.fc_offset.bwd_weight, v4(doff), v4(offset_t.view(N, -1)), sp)
+    doffset_t = ops.gemm_nt(doff, net.fc_offset.wt).view(offset_t.shape)
+    ops.deform_psroi_bwd(doffset_t, feat, rois, None, no_trans=True, data_diff=dfeat, **ps)
+    dfeat = ops.relu_bwd(feat, dfeat)
+    hw = (x.shape[1], x.shape[2])
+    W(net.conv_new_1.bwd_weight, dfeat, x, sp)
+    dx = net.conv_new_1.bwd_data(dfeat, hw)
+    W(net.rpn_head.bwd_weight, dhead, rpn, sp)
+    drpn = ops.relu_bwd(rpn, net.rpn_head.bwd_data(dhead, hw))
+    W(net.rpn_conv.bwd_weight, drpn, x, sp)
+    return net.rpn_conv.bwd_data(drpn, hw, out=dx, residual=dx)
+
+
+# ------------------------------------------------------------------------------------------------
 class SniperResNet101:
     """get_symbol_rcnn(cfg, is_train=True) as an executable object (resnet_mx_101_e2e.py:227-345)."""
 
@@ -484,7 +580,6 @@ class SniperResNet101:
         self.device = device
         cfg.wsched = WgradScheduler(bool(cfg.wgrad_stream))
         self._wt_table = None
-        self._bn_table = None
         P = self.P = ParamStore()
         fl = cfg.filter_list
         # ---- frozen stem: bn_data, conv0, bn0 (resnetc4 :402-408)
@@ -638,13 +733,11 @@ class SniperResNet101:
     def train_bns(self):
         return [b for u in self.units if not u.frozen for b in u.bns()]
 
+    def head_convs(self):
+        return [self.rpn_conv, self.rpn_head, self.conv_new_1, self.fc_offset, self.fc_new_1, self.fc_new_2, self.fc_out]
+
     def trainable_convs(self):
-        cs = []
-        for u in self.units:
-            if not u.frozen:
-                cs += u.convs()
-        cs += [self.rpn_conv, self.rpn_head, self.conv_new_1, self.fc_offset, self.fc_new_1, self.fc_new_2, self.fc_out]
-        return cs + self.af_convs
+        return [c for u in self.units if not u.frozen for c in u.convs()] + self.head_convs() + self.af_convs
 
     # ---------------------------------------------------------------- one training step
     def forward_backward(self, batch, on_bucket=None):
@@ -668,7 +761,6 @@ class SniperResNet101:
         the reference's Group([rpn_cls_prob, rpn_bbox_loss, cls_prob, bbox_loss, label]) (:338) as a dict."""
         cfg = self.cfg
         P = self.P
-        A = cfg.num_anchors
         data = batch["data"]
         B = data.shape[0]
         n1, n2, n3, n4 = cfg.units
@@ -690,22 +782,13 @@ class SniperResNet101:
         lowp = bool(cfg.bf16)
         x = self.stem(data)                                             # the reference's Cast sits right after conv0
         x = ops.maxpool3x3s2(x)
-        Hf = data.shape[2] // cfg.feat_stride
-        # Concat(c4, c5): fp32.  fp32 mode: the two producing convs write their channel slices in place.  Mixed
-        # precision: c4 / c5 are bf16 tensors and the reference's Cast(relu1, float32) (:250-252) fills the slices.
-        cat = torch.empty(B, Hf, Hf, 3072, device=data.device)
+        Hf, Wf = data.shape[2] // cfg.feat_stride, data.shape[3] // cfg.feat_stride
+        cat = torch.empty(B, Hf, Wf, 3072, device=data.device)
         last3 = n1 + n2 + n3 - 1
         has_stats = False
-        c4 = None
         for i, u in enumerate(self.units):
-            out = None
-            if not lowp:
-                if i == last3:
-                    out = cat[..., :1024]
-                elif i == len(self.units) - 1:
-                    out = cat[..., 1024:]
             nxt = self.units[i + 1].bn1 if i + 1 < len(self.units) else None
-            x = u.fwd(x, cfg, out=out, x_has_stats=has_stats, next_bn=nxt)
+            x = u.fwd(x, cfg, out=self._cat_slice(cat, i), x_has_stats=has_stats, next_bn=nxt)
             has_stats = nxt is not None and not nxt.frozen
             if i == last3:
                 c4 = x
@@ -717,29 +800,9 @@ class SniperResNet101:
         rpn = self.rpn_conv.fwd(cat, relu=True)
         head = self.rpn_head.fwd(rpn)                                      # [B,H,W,128]: 4A deltas | 2A scores
         feat = self.conv_new_1.fwd(cat, relu=True)
-        dhead = torch.zeros_like(head)
-        prob = torch.empty(B, Hf, Hf, 2 * A, device=data.device)
-        ops.count_valid(batch["label"], self.cnt_buf[0:1])
-        ops.rpn_softmax_loss(head[..., 4 * A:6 * A], batch["label"], A, cfg.grad_scale, self.cnt_buf[0:1], prob,
-                             dhead[..., 4 * A:6 * A], self.loss_buf[0:1])
-        ops.rpn_smooth_l1_loss(head, batch["bbox_target"], batch["bbox_weight"], 4 * A,
-                               3.0 * cfg.grad_scale / float(cfg.batch_images * cfg.rpn_batch_size), dhead,
-                               self.loss_buf[1:2])
-        # ---- proposals + targets, all on device
-        rois, label, bbox_target, bbox_weight = ops.multi_proposal_target(
-            prob, head, batch["im_info"], batch["gt_boxes"], batch["valid_ranges"], feat_stride=cfg.feat_stride,
-            scales=cfg.scales, ratios=cfg.ratios, rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, layout=ops.NHWC)
+        prob, dhead, rois, label, bbox_target, bbox_weight = rpn_train(self, batch, head)
         N = rois.shape[0]
-        # ---- R-FCN head
-        ps = dict(spatial_scale=1.0 / cfg.feat_stride, output_dim=256, group_size=1, pooled_size=7, part_size=7,
-                  sample_per_part=4, layout=ops.NHWC)
-        offset_t, _, _ = ops.deform_psroi_fwd(feat, rois, None, no_trans=True, want_count=False, **ps)
-        off = ops.gemm_nt(offset_t.view(N, -1), self.fc_offset.w, bias=self.fc_offset.b)          # [N,128], 98 used
-        trans = off[:, :98].contiguous().view(N, 2, 7, 7)
-        pooled, _, _ = ops.deform_psroi_fwd(feat, rois, trans, no_trans=False, trans_std=0.1, want_count=False, **ps)
-        fc1 = ops.gemm_nt(pooled.view(N, -1), self.fc_new_1.w, bias=self.fc_new_1.b, relu=True)
-        fc2 = ops.gemm_nt(fc1, self.fc_new_2.w, bias=self.fc_new_2.b, relu=True)
-        out = ops.gemm_nt(fc2, self.fc_out.w, bias=self.fc_out.b)                                  # [N,96]
+        out, rfcn = rfcn_fwd(self, feat, rois)                                                     # [N,96]
         K = cfg.num_classes
         dout = torch.zeros_like(out)
         cls_prob = torch.empty(N, K, device=data.device)
@@ -758,36 +821,15 @@ class SniperResNet101:
             f3 = c3.fwd(f2, relu=True)
             fo = co.fwd(f3)                                                  # [B,H,W,32], 2 used
             dfo = torch.zeros_like(fo)
-            scale_prob = torch.empty(B, Hf, Hf, 2, device=data.device)
+            scale_prob = torch.empty(B, Hf, Wf, 2, device=data.device)
             ops.count_valid(slab, self.cnt_buf[2:3])
             ops.rpn_softmax_loss(fo[..., :2], slab, 1, cfg.grad_scale, self.cnt_buf[2:3], scale_prob, dfo[..., :2],
                                  self.loss_buf[4:5])
             ops.focus_acc(scale_prob, slab, self.loss_buf[5:7])
 
         # ================= backward =================
-        sp = cfg.wgrad_splits
-        W = cfg.wsched
-        v4 = lambda t: t.view(1, 1, t.shape[0], t.shape[1])
-        W(self.fc_out.bwd_weight, v4(dout), v4(fc2), sp)
-        dfc2 = ops.relu_bwd(fc2, ops.gemm_nt(dout, self.fc_out.wt))
-        W(self.fc_new_2.bwd_weight, v4(dfc2), v4(fc1), sp)
-        dfc1 = ops.relu_bwd(fc1, ops.gemm_nt(dfc2, self.fc_new_2.wt))
-        W(self.fc_new_1.bwd_weight, v4(dfc1), v4(pooled.view(N, -1)), sp)
-        dpooled = ops.gemm_nt(dfc1, self.fc_new_1.wt).view(pooled.shape)
-        dfeat, dtrans = ops.deform_psroi_bwd(dpooled, feat, rois, trans, no_trans=False, trans_std=0.1, **ps)
-        doff = torch.zeros_like(off)
-        doff[:, :98] = dtrans.view(N, 98)
-        W(self.fc_offset.bwd_weight, v4(doff), v4(offset_t.view(N, -1)), sp)
-        doffset_t = ops.gemm_nt(doff, self.fc_offset.wt).view(offset_t.shape)
-        ops.deform_psroi_bwd(doffset_t, feat, rois, None, no_trans=True, data_diff=dfeat, **ps)
-        dfeat = ops.relu_bwd(feat, dfeat)
-        hw = (Hf, Hf)
-        W(self.conv_new_1.bwd_weight, dfeat, cat, sp)
-        dcat = self.conv_new_1.bwd_data(dfeat, hw)
-        W(self.rpn_head.bwd_weight, dhead, rpn, sp)
-        drpn = ops.relu_bwd(rpn, self.rpn_head.bwd_data(dhead, hw))
-        W(self.rpn_conv.bwd_weight, drpn, cat, sp)
-        dcat = self.rpn_conv.bwd_data(drpn, hw, out=dcat, residual=dcat)
+        sp, W, hw = cfg.wgrad_splits, cfg.wsched, (Hf, Wf)
+        dcat = head_bwd(self, cat, rpn, dhead, dout, rfcn)
         if self.af_convs:       # no BlockGrad in the reference: the branch's gradient flows into relu1
             W(co.bwd_weight, dfo, f3, sp)
             df3 = ops.relu_bwd(f3, co.bwd_data(dfo, hw))
@@ -815,31 +857,40 @@ class SniperResNet101:
                 self.step_count += 1
             yield out
 
-    def forward_inference(self, data, im_info, suppress_anchor_types=False, autofocus=False):
-        """get_symbol_rcnn(cfg, is_train=False) (resnet_mx_101_e2e.py:227-345 with the test branch :258-266, 321-326):
-        backbone with moving-statistics BN -> RPN -> MultiProposal (device inference proposal op) -> deformable
-        R-FCN head -> (rois [B*R,5], rpn scores [B*R], cls_prob [B*R,K], bbox_pred [B*R,4]).  No parameter is touched."""
+    def _cat_slice(self, cat, i):
+        """Concat(c4, c5) is fp32; fp32 mode: the slice unit i writes in place (c4 / c5, else None).  Mixed
+        precision: None; c4 / c5 are bf16 and the reference's Cast(relu1, float32) (:250-252) fills the slices after
+        the unit loop."""
+        i4 = sum(self.cfg.units[:3]) - 1
+        if self.cfg.bf16 or i not in (i4, len(self.units) - 1):
+            return None
+        return cat[..., :1024] if i == i4 else cat[..., 1024:]
+
+    def backbone_infer(self, data):
+        """The inference backbone: every BatchNorm on its moving statistics, folded into the convolution epilogues ->
+        the fp32 concat [B,Hf,Wf,3072]."""
         cfg = self.cfg
-        A = cfg.num_anchors
-        B = data.shape[0]
         for b in self.train_bns():
             ops.bn_frozen(b.st, cfg.bn_eps)        # scale/shift from the moving statistics (the next training step
         x = self.stem(data)                                               # recomputes them from batch statistics)
         x = ops.maxpool3x3s2(x)
-        n1, n2, n3, n4 = cfg.units
         Hf, Wf = data.shape[2] // cfg.feat_stride, data.shape[3] // cfg.feat_stride
-        cat = torch.empty(B, Hf, Wf, 3072, device=data.device)
-        last3 = n1 + n2 + n3 - 1
-        lowp = bool(cfg.bf16)
+        cat = torch.empty(data.shape[0], Hf, Wf, 3072, device=data.device)
+        last3 = sum(cfg.units[:3]) - 1
         for i, u in enumerate(self.units):
-            out = None
-            if not lowp:
-                out = cat[..., :1024] if i == last3 else (cat[..., 1024:] if i == len(self.units) - 1 else None)
-            x = u.fwd_infer(x, cfg, out=out)
-            if lowp and i == last3:
-                ops.cast_rows(x, out=cat[..., :1024])
-        if lowp:
+            x = u.fwd_infer(x, cfg, out=self._cat_slice(cat, i))
+            if i == last3:
+                c4 = x
+        if cfg.bf16:
+            ops.cast_rows(c4, out=cat[..., :1024])
             ops.cast_rows(x, out=cat[..., 1024:])
+        return cat
+
+    def forward_inference(self, data, im_info, suppress_anchor_types=False, autofocus=False):
+        """get_symbol_rcnn(cfg, is_train=False) (resnet_mx_101_e2e.py:227-345 with the test branch :258-266, 321-326):
+        backbone with moving-statistics BN -> RPN -> MultiProposal (device inference proposal op) -> deformable
+        R-FCN head -> (rois [B*R,5], rpn scores [B*R], cls_prob [B*R,K], bbox_pred [B*R,4]).  No parameter is touched."""
+        cat = self.backbone_infer(data)
         rpn = self.rpn_conv.fwd(cat, relu=True)
         head = self.rpn_head.fwd(rpn)
         feat = self.conv_new_1.fwd(cat, relu=True)
@@ -848,73 +899,19 @@ class SniperResNet101:
             if self.af is None:
                 raise RuntimeError("forward_inference(autofocus=True): call enable_autofocus() first")
             fmap = self.focus_map(cat)
-        prob = torch.empty(B, Hf, Wf, 2 * A, device=data.device)
-        ignore = torch.full((B, A * Hf * Wf), -1.0, device=data.device)
-        cnt = torch.ones(1, dtype=torch.int32, device=data.device)
-        loss = torch.zeros(1, device=data.device)
-        ops.rpn_softmax_loss(head[..., 4 * A:6 * A], ignore, A, 1.0, cnt, prob, None, loss)
-        rois, scores = ops.multi_proposal(prob, head, im_info, feat_stride=cfg.feat_stride, scales=cfg.scales,
-                                          ratios=cfg.ratios, rpn_post_nms_top_n=cfg.rpn_post_nms_top_n,
-                                          suppress_anchor_types=suppress_anchor_types, layout=ops.NHWC)
-        N = rois.shape[0]
-        ps = dict(spatial_scale=1.0 / cfg.feat_stride, output_dim=256, group_size=1, pooled_size=7, part_size=7,
-                  sample_per_part=4, layout=ops.NHWC)
-        offset_t, _, _ = ops.deform_psroi_fwd(feat, rois, None, no_trans=True, want_count=False, **ps)
-        off = ops.gemm_nt(offset_t.view(N, -1), self.fc_offset.w, bias=self.fc_offset.b)
-        trans = off[:, :98].contiguous().view(N, 2, 7, 7)
-        pooled, _, _ = ops.deform_psroi_fwd(feat, rois, trans, no_trans=False, trans_std=0.1, want_count=False, **ps)
-        fc1 = ops.gemm_nt(pooled.view(N, -1), self.fc_new_1.w, bias=self.fc_new_1.b, relu=True)
-        fc2 = ops.gemm_nt(fc1, self.fc_new_2.w, bias=self.fc_new_2.b, relu=True)
-        out = ops.gemm_nt(fc2, self.fc_out.w, bias=self.fc_out.b)
-        K = cfg.num_classes
-        cls_prob = torch.empty(N, K, device=data.device)
-        lab = torch.full((N,), -1.0, device=data.device)
-        ops.softmax_ce(out, lab, K, 1.0, cnt, cls_prob, None, loss)
-        if autofocus:
-            return rois, scores, cls_prob, out[:, K:K + 4], fmap
-        return rois, scores, cls_prob, out[:, K:K + 4]
+        res = rfcn_detect(self, head, feat, im_info, suppress_anchor_types=suppress_anchor_types)
+        return res + (fmap,) if autofocus else res
 
     def forward_rpn(self, data, im_info, suppress_anchor_types=False):
         """get_symbol_rpn(cfg, is_train=False) (resnet_mx_101_e2e.py:157-225): backbone with moving-statistics BatchNorm ->
         RPN head -> MultiProposal -> (rois [B*R,5], rpn scores [B*R]); the proposal-extraction half of
         `forward_inference` (same launches up to the proposal operator)."""
-        cfg = self.cfg
-        A = cfg.num_anchors
-        B = data.shape[0]
-        for b in self.train_bns():
-            ops.bn_frozen(b.st, cfg.bn_eps)
-        x = self.stem(data)
-        x = ops.maxpool3x3s2(x)
-        n1, n2, n3, n4 = cfg.units
-        Hf, Wf = data.shape[2] // cfg.feat_stride, data.shape[3] // cfg.feat_stride
-        cat = torch.empty(B, Hf, Wf, 3072, device=data.device)
-        last3 = n1 + n2 + n3 - 1
-        lowp = bool(cfg.bf16)
-        for i, u in enumerate(self.units):
-            out = None
-            if not lowp:
-                out = cat[..., :1024] if i == last3 else (cat[..., 1024:] if i == len(self.units) - 1 else None)
-            x = u.fwd_infer(x, cfg, out=out)
-            if lowp and i == last3:
-                ops.cast_rows(x, out=cat[..., :1024])
-        if lowp:
-            ops.cast_rows(x, out=cat[..., 1024:])
-        rpn = self.rpn_conv.fwd(cat, relu=True)
-        head = self.rpn_head.fwd(rpn)
-        prob = torch.empty(B, Hf, Wf, 2 * A, device=data.device)
-        ignore = torch.full((B, A * Hf * Wf), -1.0, device=data.device)
-        cnt = torch.ones(1, dtype=torch.int32, device=data.device)
-        loss = torch.zeros(1, device=data.device)
-        ops.rpn_softmax_loss(head[..., 4 * A:6 * A], ignore, A, 1.0, cnt, prob, None, loss)
-        return ops.multi_proposal(prob, head, im_info, feat_stride=cfg.feat_stride, scales=cfg.scales, ratios=cfg.ratios,
-                                  rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, suppress_anchor_types=suppress_anchor_types,
-                                  layout=ops.NHWC)
+        head = self.rpn_head.fwd(self.rpn_conv.fwd(self.backbone_infer(data), relu=True))
+        return rpn_proposals(self, head, im_info, suppress_anchor_types=suppress_anchor_types)[:2]
 
     # ---------------------------------------------------------------- reference checkpoints (utils.py:45-100)
     def _named_convs(self):
-        cs = [c for u in self.units for c in u.convs()]
-        return cs + [self.rpn_conv, self.rpn_head, self.conv_new_1, self.fc_offset, self.fc_new_1, self.fc_new_2,
-                     self.fc_out] + self.af_convs
+        return [c for u in self.units for c in u.convs()] + self.head_convs() + self.af_convs
 
     def _named_bns(self):
         return [self.bn_data, self.bn0] + [b for u in self.units for b in u.bns()]

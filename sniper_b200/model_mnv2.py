@@ -29,7 +29,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .model import Cfg, Conv, ParamStore, WgradScheduler
+from .model import Cfg, Conv, ParamStore, WgradScheduler, head_bwd, rfcn_detect, rfcn_fwd, rpn_train
 
 
 def pad64(c):
@@ -267,9 +267,7 @@ class SniperMobileNetV2:
         this configuration -- data [B,3,512,512], label [B, 15*16*16], bbox_target / bbox_weight [B,60,16,16], gt_boxes
         [B,100,5], valid_ranges [B,2], im_info [B,3] (`crowd_boxes` of the symbol is not read by the operator)."""
         cfg, P = self.cfg, self.P
-        A = cfg.num_anchors
         data = batch["data"]
-        B = data.shape[0]
         dev = data.device
         lowp = bool(cfg.bf16)
         P.g.zero_()
@@ -291,34 +289,14 @@ class SniperMobileNetV2:
         cl = self.last.fwd(x, stats=self.bn_last.st.sums)
         al = self.bn_last.fwd(cl, cfg, have_stats=True)
         feat_in = ops.cast_rows(al, torch.float32) if lowp else al                    # Cast(float32) (:226)
-        Hf = data.shape[2] // cfg.feat_stride
 
         # ---- RPN (get_rpn) + conv_new_1
         rpn = self.rpn_conv.fwd(feat_in, relu=True)
         head = self.rpn_head.fwd(rpn)                                     # [B,H,W,96]: 4A deltas | 2A scores
         feat = self.conv_new_1.fwd(feat_in, relu=True)
-        dhead = torch.zeros_like(head)
-        prob = torch.empty(B, Hf, Hf, 2 * A, device=dev)
-        ops.count_valid(batch["label"], self.cnt_buf[0:1])
-        ops.rpn_softmax_loss(head[..., 4 * A:6 * A], batch["label"], A, cfg.grad_scale, self.cnt_buf[0:1], prob,
-                             dhead[..., 4 * A:6 * A], self.loss_buf[0:1])
-        ops.rpn_smooth_l1_loss(head, batch["bbox_target"], batch["bbox_weight"], 4 * A,
-                               3.0 * cfg.grad_scale / float(cfg.batch_images * cfg.rpn_batch_size), dhead,
-                               self.loss_buf[1:2])
-        rois, label, bbox_target, bbox_weight = ops.multi_proposal_target(
-            prob, head, batch["im_info"], batch["gt_boxes"], batch["valid_ranges"], feat_stride=cfg.feat_stride,
-            scales=cfg.scales, ratios=cfg.ratios, rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, layout=ops.NHWC)
+        prob, dhead, rois, label, bbox_target, bbox_weight = rpn_train(self, batch, head)
         N = rois.shape[0]
-        # ---- R-FCN head
-        ps = dict(spatial_scale=1.0 / cfg.feat_stride, output_dim=256, group_size=1, pooled_size=7, part_size=7,
-                  sample_per_part=4, layout=ops.NHWC)
-        offset_t, _, _ = ops.deform_psroi_fwd(feat, rois, None, no_trans=True, want_count=False, **ps)
-        off = ops.gemm_nt(offset_t.view(N, -1), self.fc_offset.w, bias=self.fc_offset.b)          # [N,128], 98 used
-        trans = off[:, :98].contiguous().view(N, 2, 7, 7)
-        pooled, _, _ = ops.deform_psroi_fwd(feat, rois, trans, no_trans=False, trans_std=0.1, want_count=False, **ps)
-        fc1 = ops.gemm_nt(pooled.view(N, -1), self.fc_new_1.w, bias=self.fc_new_1.b, relu=True)
-        fc2 = ops.gemm_nt(fc1, self.fc_new_2.w, bias=self.fc_new_2.b, relu=True)
-        out = ops.gemm_nt(fc2, self.fc_out.w, bias=self.fc_out.b)                                  # [N,96]
+        out, rfcn = rfcn_fwd(self, feat, rois)                                                     # [N,96]
         K = cfg.num_classes
         dout = torch.zeros_like(out)
         cls_prob = torch.empty(N, K, device=dev)
@@ -331,27 +309,7 @@ class SniperMobileNetV2:
         # ================= backward =================
         sp = cfg.wgrad_splits
         W = cfg.wsched
-        v4 = lambda t: t.view(1, 1, t.shape[0], t.shape[1])
-        W(self.fc_out.bwd_weight, v4(dout), v4(fc2), sp)
-        dfc2 = ops.relu_bwd(fc2, ops.gemm_nt(dout, self.fc_out.wt))
-        W(self.fc_new_2.bwd_weight, v4(dfc2), v4(fc1), sp)
-        dfc1 = ops.relu_bwd(fc1, ops.gemm_nt(dfc2, self.fc_new_2.wt))
-        W(self.fc_new_1.bwd_weight, v4(dfc1), v4(pooled.view(N, -1)), sp)
-        dpooled = ops.gemm_nt(dfc1, self.fc_new_1.wt).view(pooled.shape)
-        dfeat, dtrans = ops.deform_psroi_bwd(dpooled, feat, rois, trans, no_trans=False, trans_std=0.1, **ps)
-        doff = torch.zeros_like(off)
-        doff[:, :98] = dtrans.view(N, 98)
-        W(self.fc_offset.bwd_weight, v4(doff), v4(offset_t.view(N, -1)), sp)
-        doffset_t = ops.gemm_nt(doff, self.fc_offset.wt).view(offset_t.shape)
-        ops.deform_psroi_bwd(doffset_t, feat, rois, None, no_trans=True, data_diff=dfeat, **ps)
-        dfeat = ops.relu_bwd(feat, dfeat)
-        hw = (Hf, Hf)
-        W(self.conv_new_1.bwd_weight, dfeat, feat_in, sp)
-        dfi = self.conv_new_1.bwd_data(dfeat, hw)
-        W(self.rpn_head.bwd_weight, dhead, rpn, sp)
-        drpn = ops.relu_bwd(rpn, self.rpn_head.bwd_data(dhead, hw))
-        W(self.rpn_conv.bwd_weight, drpn, feat_in, sp)
-        dfi = self.rpn_conv.bwd_data(drpn, hw, out=dfi, residual=dfi)
+        dfi = head_bwd(self, feat_in, rpn, dhead, dout, rfcn)
         g = ops.cast_rows(dfi, torch.bfloat16) if lowp else dfi                  # backward of the Cast
         # ---- backbone backward
         dcl = self.bn_last.bwd(cl, g)
@@ -375,9 +333,6 @@ class SniperMobileNetV2:
         deformable R-FCN head -> (rois [B*R,5], rpn scores [B*R], cls_prob [B*R,K], bbox_pred [B*R,4]).  No parameter is
         touched.  BatchNorm + clip run as one `sniper_affine_act` pass per layer (the GEMM epilogue has ReLU, not clip)."""
         cfg = self.cfg
-        A = cfg.num_anchors
-        B = data.shape[0]
-        dev = data.device
         lowp = bool(cfg.bf16)
         for b in self.all_bns():
             ops.bn_frozen(b.st, cfg.bn_eps)            # scale / shift from the moving statistics (the next training
@@ -393,33 +348,10 @@ class SniperMobileNetV2:
             x = y
         al = act(self.bn_last, self.last.fwd(x))
         feat_in = ops.cast_rows(al, torch.float32) if lowp else al
-        Hf, Wf = data.shape[2] // cfg.feat_stride, data.shape[3] // cfg.feat_stride
         rpn = self.rpn_conv.fwd(feat_in, relu=True)
         head = self.rpn_head.fwd(rpn)
         feat = self.conv_new_1.fwd(feat_in, relu=True)
-        prob = torch.empty(B, Hf, Wf, 2 * A, device=dev)
-        ignore = torch.full((B, A * Hf * Wf), -1.0, device=dev)
-        cnt = torch.ones(1, dtype=torch.int32, device=dev)
-        loss = torch.zeros(1, device=dev)
-        ops.rpn_softmax_loss(head[..., 4 * A:6 * A], ignore, A, 1.0, cnt, prob, None, loss)
-        rois, scores = ops.multi_proposal(prob, head, im_info, feat_stride=cfg.feat_stride, scales=cfg.scales,
-                                          ratios=cfg.ratios, rpn_pre_nms_top_n=rpn_pre_nms_top_n,
-                                          rpn_post_nms_top_n=cfg.rpn_post_nms_top_n, layout=ops.NHWC)
-        N = rois.shape[0]
-        ps = dict(spatial_scale=1.0 / cfg.feat_stride, output_dim=256, group_size=1, pooled_size=7, part_size=7,
-                  sample_per_part=4, layout=ops.NHWC)
-        offset_t, _, _ = ops.deform_psroi_fwd(feat, rois, None, no_trans=True, want_count=False, **ps)
-        off = ops.gemm_nt(offset_t.view(N, -1), self.fc_offset.w, bias=self.fc_offset.b)
-        trans = off[:, :98].contiguous().view(N, 2, 7, 7)
-        pooled, _, _ = ops.deform_psroi_fwd(feat, rois, trans, no_trans=False, trans_std=0.1, want_count=False, **ps)
-        fc1 = ops.gemm_nt(pooled.view(N, -1), self.fc_new_1.w, bias=self.fc_new_1.b, relu=True)
-        fc2 = ops.gemm_nt(fc1, self.fc_new_2.w, bias=self.fc_new_2.b, relu=True)
-        out = ops.gemm_nt(fc2, self.fc_out.w, bias=self.fc_out.b)
-        K = cfg.num_classes
-        cls_prob = torch.empty(N, K, device=dev)
-        lab = torch.full((N,), -1.0, device=dev)
-        ops.softmax_ce(out, lab, K, 1.0, cnt, cls_prob, None, loss)
-        return rois, scores, cls_prob, out[:, K:K + 4]
+        return rfcn_detect(self, head, feat, im_info, rpn_pre_nms_top_n=rpn_pre_nms_top_n)
 
     # ---------------------------------------------------------------- optimizer
     def set_lr(self, lr=None):
