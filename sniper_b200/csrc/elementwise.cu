@@ -873,6 +873,34 @@ int resident_blocks(K kernel) {
 }  // namespace
 
 namespace {
+// Argument checks of the entry points, made BEFORE any CUDA call: the kernels read and write whole 16-byte (row-blocked
+// kernels, fp32 flat kernels) or 8-byte (bf16 in the flat ld4 / st4 kernels) vectors, so a base pointer or a row
+// stride that is not a whole number of vectors would be a misaligned-address fault on the device, not an error code.
+// `what` names the argument in the message.
+int check_rows(const char* fn, const char* what, const void* p, long ld, int C, int vec, int bytes) {
+  SN_CHECK(p != nullptr, "%s: %s is null", fn, what);
+  SN_CHECK(((uintptr_t)p & (uintptr_t)(bytes - 1)) == 0, "%s: %s must be %d-byte aligned", fn, what, bytes);
+  SN_CHECK(ld % vec == 0, "%s: row stride of %s (%ld) must be a multiple of %d", fn, what, ld, vec);
+  SN_CHECK(ld >= C, "%s: row stride of %s (%ld) is smaller than C (%d)", fn, what, ld, C);
+  return 0;
+}
+// per-channel fp32 vector read with float4 loads
+int check_chan(const char* fn, const char* what, const void* p) {
+  SN_CHECK(p != nullptr, "%s: %s is null", fn, what);
+  SN_CHECK(((uintptr_t)p & 15) == 0, "%s: %s must be 16-byte aligned", fn, what);
+  return 0;
+}
+int check_shape(const char* fn, long M, int C, int vec) {
+  SN_CHECK(M >= 0, "%s: M (%ld) must not be negative", fn, M);
+  SN_CHECK(C > 0 && C % vec == 0, "%s: C (%d) must be a positive multiple of %d", fn, C, vec);
+  return 0;
+}
+int check_dtype(const char* fn, int dtype) {
+  SN_CHECK(dtype == 0 || dtype == 1, "%s: dtype must be 0 (fp32) or 1 (bf16)", fn);
+  return 0;
+}
+#define SN_TRY(call) do { if (call) return -1; } while (0)
+
 template <typename T, int ACT>
 int bn_act_bwd_launch(const void* x, long ldx, const void* dy, long lddy, const float* scale, const float* shift,
                       const float* mean, const float* invstd, double* sums, const void* add, long ldadd, void* dx,
@@ -895,9 +923,14 @@ extern "C" {
 // dtype (here and below): storage type of the activation tensors, 0 = fp32, 1 = bf16 (arithmetic is fp32 either way)
 int sniper_affine_act(const void* x, long ldx, const float* scale, const float* shift, void* y, long ldy, long M,
                       int C, int relu, int dtype, void* stream) {
-  SN_CHECK(C % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0, "affine_act: C/ld must be multiples of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "affine_act: dtype must be 0 (fp32) or 1 (bf16)");
-  SN_CHECK(dtype == 0 || (C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0), "affine_act: bf16 needs C/ld multiples of 8");
+  SN_TRY(check_dtype("affine_act", dtype));
+  const int vec = dtype == 0 ? 4 : 8;
+  SN_TRY(check_shape("affine_act", M, C, vec));
+  SN_TRY(check_rows("affine_act", "x", x, ldx, C, vec, 16));
+  SN_TRY(check_rows("affine_act", "y", y, ldy, C, vec, 16));
+  SN_TRY(check_chan("affine_act", "scale", scale));
+  SN_TRY(check_chan("affine_act", "shift", shift));
+  if (M == 0) return 0;
   const RowBlock rb = dtype == 0 ? row_block(M, C, 4, resident_blocks(affine_act_kernel<float>))
                                  : row_block(M, C, 8, resident_blocks(affine_act_kernel<bf16>));
   if (dtype == 0)
@@ -917,9 +950,13 @@ int sniper_affine_act(const void* x, long ldx, const float* scale, const float* 
 int sniper_bn_stats(const void* x, long ldx, long M, int C, const float* gamma, const float* beta, float eps,
                     float momentum, int fix_gamma, float* moving_mean, float* moving_var, double* sums, float* mean,
                     float* invstd, float* scale, float* shift, int dtype, void* stream) {
-  SN_CHECK(C % 4 == 0 && ldx % 4 == 0, "bn_stats: C/ld must be multiples of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "bn_stats: dtype must be 0 (fp32) or 1 (bf16)");
-  SN_CHECK(dtype == 0 || (C % 8 == 0 && ldx % 8 == 0), "bn_stats: bf16 needs C/ld multiples of 8");
+  SN_TRY(check_dtype("bn_stats", dtype));
+  const int vec = dtype == 0 ? 4 : 8;
+  SN_TRY(check_shape("bn_stats", M, C, vec));
+  SN_TRY(check_rows("bn_stats", "x", x, ldx, C, vec, 16));
+  SN_CHECK(sums != nullptr && ((uintptr_t)sums & 7) == 0, "bn_stats: sums must be a non-null, 8-byte aligned double[2C]");
+  SN_CHECK((moving_mean == nullptr) == (moving_var == nullptr), "bn_stats: moving_mean and moving_var go together");
+  SN_CHECK(M >= 1, "bn_stats: M (%ld) must be at least 1 (statistics of no rows are undefined)", M);
   int rc;
   if (dtype == 0)
     rc = launch_colsum<0, float>((cudaStream_t)stream, static_cast<const float*>(x), ldx, nullptr, 0, nullptr, nullptr,
@@ -940,6 +977,12 @@ int sniper_bn_stats(const void* x, long ldx, long M, int C, const float* gamma, 
 int sniper_bn_finalize(double* sums, long M, int C, const float* gamma, const float* beta, float eps, float momentum,
                        int fix_gamma, float* moving_mean, float* moving_var, float* mean, float* invstd, float* scale,
                        float* shift, void* stream) {
+  SN_CHECK(C > 0, "bn_finalize: C (%d) must be positive", C);
+  SN_CHECK(M >= 0, "bn_finalize: M (%ld) must not be negative", M);
+  SN_CHECK(sums != nullptr && ((uintptr_t)sums & 7) == 0, "bn_finalize: sums must be a non-null, 8-byte aligned double[2C]");
+  SN_CHECK(mean && invstd && scale && shift, "bn_finalize: mean / invstd / scale / shift must not be null");
+  SN_CHECK((moving_mean == nullptr) == (moving_var == nullptr), "bn_finalize: moving_mean and moving_var go together");
+  SN_CHECK(M >= 1, "bn_finalize: M (%ld) must be at least 1 (statistics of no rows are undefined)", M);
   bn_finalize_kernel<<<sn::div_up(C, 128), 128, 0, (cudaStream_t)stream>>>(sums, M, C, gamma, beta, eps, momentum,
                                                                           fix_gamma, moving_mean, moving_var, mean,
                                                                           invstd, scale, shift);
@@ -953,9 +996,16 @@ int sniper_bn_apply_train(const void* x, long ldx, const double* sums, long M, i
                           const float* beta, float eps, float momentum, int fix_gamma, float* moving_mean,
                           float* moving_var, float* mean, float* invstd, float* scale, float* shift, void* y, long ldy,
                           int relu, int dtype, void* stream) {
-  SN_CHECK(C % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0, "bn_apply_train: C/ld must be multiples of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "bn_apply_train: dtype must be 0 (fp32) or 1 (bf16)");
-  SN_CHECK(dtype == 0 || (C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0), "bn_apply_train: bf16 needs C/ld multiples of 8");
+  SN_TRY(check_dtype("bn_apply_train", dtype));
+  const int vec = dtype == 0 ? 4 : 8;
+  SN_TRY(check_shape("bn_apply_train", M, C, vec));
+  SN_TRY(check_rows("bn_apply_train", "x", x, ldx, C, vec, 16));
+  SN_TRY(check_rows("bn_apply_train", "y", y, ldy, C, vec, 16));
+  SN_CHECK(sums != nullptr && ((uintptr_t)sums & 7) == 0,
+           "bn_apply_train: sums must be a non-null, 8-byte aligned double[2C]");
+  SN_CHECK(mean && invstd && scale && shift, "bn_apply_train: mean / invstd / scale / shift must not be null");
+  SN_CHECK((moving_mean == nullptr) == (moving_var == nullptr), "bn_apply_train: moving_mean and moving_var go together");
+  SN_CHECK(M >= 1, "bn_apply_train: M (%ld) must be at least 1 (statistics of no rows are undefined)", M);
   const RowBlock rb = dtype == 0 ? row_block(M, C, 4, resident_blocks(bn_apply_train_kernel<float>))
                                  : row_block(M, C, 8, resident_blocks(bn_apply_train_kernel<bf16>));
   if (dtype == 0)
@@ -972,6 +1022,9 @@ int sniper_bn_apply_train(const void* x, long ldx, const double* sums, long M, i
 
 int sniper_bn_frozen(int C, const float* gamma, const float* beta, const float* moving_mean, const float* moving_var,
                      float eps, int fix_gamma, float* scale, float* shift, void* stream) {
+  SN_CHECK(C > 0, "bn_frozen: C (%d) must be positive", C);
+  SN_CHECK(beta && moving_mean && moving_var && scale && shift && (fix_gamma || gamma),
+           "bn_frozen: gamma / beta / moving_mean / moving_var / scale / shift must not be null");
   bn_frozen_kernel<<<sn::div_up(C, 128), 128, 0, (cudaStream_t)stream>>>(C, gamma, beta, moving_mean, moving_var, eps,
                                                                         fix_gamma, scale, shift);
   SN_LAUNCH_CHECK();
@@ -984,11 +1037,20 @@ int sniper_bn_frozen(int C, const float* gamma, const float* beta, const float* 
 int sniper_bn_act_bwd(const void* x, long ldx, const void* dy, long lddy, const float* scale, const float* shift,
                       const float* mean, const float* invstd, double* sums, const void* add, long ldadd, void* dx,
                       long lddx, float* dgamma, float* dbeta, long M, int C, int act, int dtype, void* stream) {
-  SN_CHECK(C % 4 == 0 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0, "bn_act_bwd: C/ld must be multiples of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "bn_act_bwd: dtype must be 0 (fp32) or 1 (bf16)");
+  SN_TRY(check_dtype("bn_act_bwd", dtype));
   SN_CHECK(act >= 1 && act <= 3, "bn_act_bwd: act must be 1 (relu), 2 (relu6) or 3 (none)");
-  SN_CHECK(dtype == 0 || (C % 8 == 0 && ldx % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0 && ldadd % 8 == 0),
-           "bn_act_bwd: bf16 needs C/ld multiples of 8");
+  const int vec = dtype == 0 ? 4 : 8;
+  SN_TRY(check_shape("bn_act_bwd", M, C, vec));
+  SN_TRY(check_rows("bn_act_bwd", "x", x, ldx, C, vec, 16));
+  SN_TRY(check_rows("bn_act_bwd", "dy", dy, lddy, C, vec, 16));
+  SN_TRY(check_rows("bn_act_bwd", "dx", dx, lddx, C, vec, 16));
+  if (add) SN_TRY(check_rows("bn_act_bwd", "add", add, ldadd, C, vec, 16));
+  SN_TRY(check_chan("bn_act_bwd", "scale", scale));
+  SN_TRY(check_chan("bn_act_bwd", "shift", shift));
+  SN_TRY(check_chan("bn_act_bwd", "mean", mean));
+  SN_TRY(check_chan("bn_act_bwd", "invstd", invstd));
+  SN_CHECK(sums != nullptr && ((uintptr_t)sums & 7) == 0, "bn_act_bwd: sums must be a non-null, 8-byte aligned double[2C]");
+  if (M == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
 #define SN_BN_BWD(T, A) rc = bn_act_bwd_launch<T, A>(x, ldx, dy, lddy, scale, shift, mean, invstd, sums, add, ldadd, dx, lddx, M, C, st)
@@ -1017,7 +1079,16 @@ int sniper_bn_relu_bwd(const void* x, long ldx, const void* dy, long lddy, const
 int sniper_affine_relu_bwd(const float* x, long ldx, const float* dy, long lddy, const float* scale,
                            const float* shift, const float* add, long ldadd, float* dx, long lddx, long M, int C,
                            int relu, void* stream) {
-  SN_CHECK(C % 4 == 0, "affine_relu_bwd: C must be a multiple of 4");
+  SN_TRY(check_shape("affine_relu_bwd", M, C, 4));
+  SN_TRY(check_rows("affine_relu_bwd", "x", x, ldx, C, 4, 16));
+  SN_TRY(check_rows("affine_relu_bwd", "dy", dy, lddy, C, 4, 16));
+  SN_TRY(check_rows("affine_relu_bwd", "dx", dx, lddx, C, 4, 16));
+  if (add) SN_TRY(check_rows("affine_relu_bwd", "add", add, ldadd, C, 4, 16));
+  SN_TRY(check_chan("affine_relu_bwd", "scale", scale));
+  SN_TRY(check_chan("affine_relu_bwd", "shift", shift));
+  // RowSplit's division path (C/4 not a power of two) splits the flat vector index in 32 bits
+  SN_CHECK(M * (C / 4) < (1L << 32), "affine_relu_bwd: M * C/4 must be below 2^32");
+  if (M == 0) return 0;
   affine_relu_bwd_kernel<<<ew_grid(M * (C / 4)), kTPB, 0, (cudaStream_t)stream>>>(x, ldx, dy, lddy, scale, shift, add,
                                                                                  ldadd, dx, lddx, M, C, relu);
   SN_LAUNCH_CHECK();
@@ -1026,8 +1097,15 @@ int sniper_affine_relu_bwd(const float* x, long ldx, const float* dy, long lddy,
 
 int sniper_relu_bwd(const void* y, long ldy, const void* dy, long lddy, void* dx, long lddx, long M, int C, int dtype,
                     void* stream) {
-  SN_CHECK(C % 4 == 0, "relu_bwd: C must be a multiple of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "relu_bwd: dtype must be 0 (fp32) or 1 (bf16)");
+  SN_TRY(check_dtype("relu_bwd", dtype));
+  SN_TRY(check_shape("relu_bwd", M, C, 4));
+  const int bytes = dtype == 0 ? 16 : 8;      // 4 channels per access in either storage type
+  SN_TRY(check_rows("relu_bwd", "y", y, ldy, C, 4, bytes));
+  SN_TRY(check_rows("relu_bwd", "dy", dy, lddy, C, 4, bytes));
+  SN_TRY(check_rows("relu_bwd", "dx", dx, lddx, C, 4, bytes));
+  // RowSplit's division path (C/4 not a power of two) splits the flat vector index in 32 bits
+  SN_CHECK(M * (C / 4) < (1L << 32), "relu_bwd: M * C/4 must be below 2^32");
+  if (M == 0) return 0;
   if (dtype == 0)
     relu_bwd_kernel<float><<<ew_grid(M * (C / 4)), kTPB, 0, (cudaStream_t)stream>>>(
         static_cast<const float*>(y), ldy, static_cast<const float*>(dy), lddy, static_cast<float*>(dx), lddx, M, C);
@@ -1040,8 +1118,11 @@ int sniper_relu_bwd(const void* y, long ldy, const void* dy, long lddy, void* dx
 
 // y[M,C] (ldy) = cast(x[M,C] (ldx)); dtypes 0 = fp32, 1 = bf16.
 int sniper_cast_rows(const void* x, long ldx, int x_dtype, void* y, long ldy, int y_dtype, long M, int C, void* stream) {
-  SN_CHECK(C % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0, "cast_rows: C/ld must be multiples of 4");
   SN_CHECK((x_dtype | y_dtype | 1) == 1, "cast_rows: dtypes must be 0 (fp32) or 1 (bf16)");
+  SN_TRY(check_shape("cast_rows", M, C, 4));
+  SN_TRY(check_rows("cast_rows", "x", x, ldx, C, 4, x_dtype == 0 ? 16 : 8));
+  SN_TRY(check_rows("cast_rows", "y", y, ldy, C, 4, y_dtype == 0 ? 16 : 8));
+  if (M == 0) return 0;
   const int g = ew_grid(M * (C / 4));
   cudaStream_t st = (cudaStream_t)stream;
   if (x_dtype == 0 && y_dtype == 0)
@@ -1057,8 +1138,12 @@ int sniper_cast_rows(const void* x, long ldx, int x_dtype, void* y, long ldy, in
 }
 
 int sniper_maxpool3x3s2_nhwc(const void* x, void* y, int NB, int H, int W, int C, int dtype, void* stream) {
-  SN_CHECK(C % 4 == 0, "maxpool: C must be a multiple of 4");
-  SN_CHECK(dtype == 0 || dtype == 1, "maxpool: dtype must be 0 (fp32) or 1 (bf16)");
+  SN_TRY(check_dtype("maxpool", dtype));
+  SN_CHECK(NB >= 0 && H > 0 && W > 0, "maxpool: NB (%d) must not be negative, H (%d) and W (%d) must be positive", NB, H, W);
+  SN_TRY(check_shape("maxpool", NB, C, 4));
+  SN_TRY(check_rows("maxpool", "x", x, C, C, 4, dtype == 0 ? 16 : 8));
+  SN_TRY(check_rows("maxpool", "y", y, C, C, 4, dtype == 0 ? 16 : 8));
+  if (NB == 0) return 0;
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const int g = ew_grid((long)NB * Ho * Wo * (C / 4));
   if (dtype == 0)
@@ -1142,7 +1227,10 @@ int sniper_colsum(const float* x, long ldx, long M, int C, float* out_accum, voi
 
 int sniper_sgd_mom(float* w, float* mom, const float* g, long n, float lr, float wd, float momentum, float rescale,
                    void* stream) {
-  SN_CHECK((((uintptr_t)w | (uintptr_t)mom | (uintptr_t)g) & 15) == 0, "sgd_mom: buffers must be 16-byte aligned");
+  SN_CHECK(n >= 0, "sgd_mom: n (%ld) must not be negative", n);
+  SN_CHECK(w && mom && g, "sgd_mom: w / mom / g must not be null");
+  SN_CHECK((((uintptr_t)w | (uintptr_t)mom | (uintptr_t)g) & 15) == 0, "sgd_mom: w / mom / g must be 16-byte aligned");
+  if (n == 0) return 0;
   sgd_mom_kernel<<<ew_grid(n / 4 + 1), kTPB, 0, (cudaStream_t)stream>>>(w, mom, g, n, lr, wd, momentum, rescale);
   SN_LAUNCH_CHECK();
   return 0;
@@ -1151,9 +1239,12 @@ int sniper_sgd_mom(float* w, float* mom, const float* g, long n, float lr, float
 // hyper: device float[2] = {lr, wd}.  w_bf16: optional bf16 copy of the updated weights (8-byte aligned).
 int sniper_sgd_mom_dev(float* w, float* mom, const float* g, long n, const float* hyper, float lr_mult, float wd_mult,
                        float momentum, float rescale, void* w_bf16, void* stream) {
-  SN_CHECK((((uintptr_t)w | (uintptr_t)mom | (uintptr_t)g) & 15) == 0, "sgd_mom_dev: buffers must be 16-byte aligned");
-  SN_CHECK(hyper != nullptr, "sgd_mom_dev: hyper (device {lr, wd}) is required");
+  SN_CHECK(n >= 0, "sgd_mom_dev: n (%ld) must not be negative", n);
+  SN_CHECK(w && mom && g, "sgd_mom_dev: w / mom / g must not be null");
+  SN_CHECK((((uintptr_t)w | (uintptr_t)mom | (uintptr_t)g) & 15) == 0, "sgd_mom_dev: w / mom / g must be 16-byte aligned");
+  SN_CHECK(hyper != nullptr && ((uintptr_t)hyper & 3) == 0, "sgd_mom_dev: hyper (device {lr, wd}) is required");
   SN_CHECK(((uintptr_t)w_bf16 & 7) == 0, "sgd_mom_dev: w_bf16 must be 8-byte aligned");
+  if (n == 0) return 0;
   sgd_mom_dev_kernel<<<ew_grid(n / 4 + 1), kTPB, 0, (cudaStream_t)stream>>>(
       w, mom, g, n, hyper, lr_mult, wd_mult, momentum, rescale, static_cast<__nv_bfloat16*>(w_bf16));
   SN_LAUNCH_CHECK();

@@ -159,6 +159,9 @@ extern "C" {
 
 // out_count must be zeroed by the caller (device int)
 int sniper_count_valid(const float* label, long n, int ignore_label, int* out_count, void* stream) {
+  SN_CHECK(n >= 0, "count_valid: n (%ld) must not be negative", n);
+  SN_CHECK(label != nullptr && out_count != nullptr, "count_valid: label / out_count must not be null");
+  if (n == 0) return 0;
   count_valid_kernel<<<lgrid(n), 256, 0, (cudaStream_t)stream>>>(label, n, ignore_label, out_count);
   SN_LAUNCH_CHECK();
   return 0;
@@ -167,6 +170,13 @@ int sniper_count_valid(const float* label, long n, int ignore_label, int* out_co
 int sniper_rpn_softmax_loss(const float* score, int ld, const float* label, int B, int H, int W, int A,
                             float grad_scale, const int* valid_cnt, float* prob, int ldp, float* dscore, int ldg,
                             float* loss_sum, void* stream) {
+  SN_CHECK(B >= 0 && H > 0 && W > 0 && A >= 1, "rpn_softmax_loss: need B >= 0, H, W > 0 and A >= 1");
+  SN_CHECK(score != nullptr && prob != nullptr, "rpn_softmax_loss: score / prob must not be null");
+  SN_CHECK(ld >= 2 * A, "rpn_softmax_loss: ld of score (%d) is smaller than 2A (%d)", ld, 2 * A);
+  SN_CHECK(ldp >= 2 * A, "rpn_softmax_loss: ld of prob (%d) is smaller than 2A (%d)", ldp, 2 * A);
+  SN_CHECK(dscore == nullptr || ldg >= 2 * A, "rpn_softmax_loss: ld of dscore (%d) is smaller than 2A (%d)", ldg, 2 * A);
+  SN_CHECK(dscore == nullptr || label != nullptr, "rpn_softmax_loss: label is null (the gradient needs it)");
+  if (B == 0) return 0;
   rpn_softmax_kernel<<<lgrid((long)B * H * W * A), 256, 0, (cudaStream_t)stream>>>(
       score, ld, label, B, H, W, A, grad_scale, valid_cnt, prob, ldp, dscore, ldg, loss_sum);
   SN_LAUNCH_CHECK();
@@ -175,6 +185,11 @@ int sniper_rpn_softmax_loss(const float* score, int ld, const float* label, int 
 
 int sniper_rpn_smooth_l1_loss(const float* pred, int ld, const float* target, const float* weight, int B, int H, int W,
                               int C4, float grad_scale, float* dpred, int ldg, float* loss_sum, void* stream) {
+  SN_CHECK(B >= 0 && H > 0 && W > 0 && C4 >= 1, "rpn_smooth_l1_loss: need B >= 0, H, W > 0 and C4 >= 1");
+  SN_CHECK(pred && target && weight && dpred, "rpn_smooth_l1_loss: pred / target / weight / dpred must not be null");
+  SN_CHECK(ld >= C4, "rpn_smooth_l1_loss: ld of pred (%d) is smaller than C4 (%d)", ld, C4);
+  SN_CHECK(ldg >= C4, "rpn_smooth_l1_loss: ld of dpred (%d) is smaller than C4 (%d)", ldg, C4);
+  if (B == 0) return 0;
   rpn_smooth_l1_kernel<<<lgrid((long)B * H * W * C4), 256, 0, (cudaStream_t)stream>>>(
       pred, ld, target, weight, B, H, W, C4, grad_scale, dpred, ldg, loss_sum);
   SN_LAUNCH_CHECK();
@@ -184,7 +199,13 @@ int sniper_rpn_smooth_l1_loss(const float* pred, int ld, const float* target, co
 int sniper_softmax_ce(const float* logits, int ld, const float* label, int N, int K, int ignore_label,
                       float grad_scale, const int* valid_cnt, float* prob, int ldp, float* grad, int ldg,
                       float* loss_sum, void* stream) {
-  SN_CHECK(K <= 4096, "softmax_ce: K too large");
+  SN_CHECK(K >= 1 && K <= 4096, "softmax_ce: K (%d) must be in [1, 4096]", K);
+  SN_CHECK(N >= 0, "softmax_ce: N (%d) must not be negative", N);
+  SN_CHECK(logits != nullptr && label != nullptr, "softmax_ce: logits / label must not be null");
+  SN_CHECK(ld >= K, "softmax_ce: ld of logits (%d) is smaller than K (%d)", ld, K);
+  SN_CHECK(prob == nullptr || ldp >= K, "softmax_ce: ld of prob (%d) is smaller than K (%d)", ldp, K);
+  SN_CHECK(grad == nullptr || ldg >= K, "softmax_ce: ld of grad (%d) is smaller than K (%d)", ldg, K);
+  if (N == 0) return 0;
   softmax_ce_kernel<<<sn::div_up((long)N * 32, 256), 256, 0, (cudaStream_t)stream>>>(
       logits, ld, label, N, K, ignore_label, grad_scale, valid_cnt, prob, ldp, grad, ldg, loss_sum);
   SN_LAUNCH_CHECK();
@@ -193,6 +214,11 @@ int sniper_softmax_ce(const float* logits, int ld, const float* label, int N, in
 
 int sniper_smooth_l1_loss(const float* pred, int ld, const float* target, const float* weight, long N, int C,
                           float grad_scale, float* grad, int ldg, float* loss_sum, void* stream) {
+  SN_CHECK(N >= 0 && C >= 1, "smooth_l1_loss: need N >= 0 and C >= 1");
+  SN_CHECK(pred && target && weight && grad, "smooth_l1_loss: pred / target / weight / grad must not be null");
+  SN_CHECK(ld >= C, "smooth_l1_loss: ld of pred (%d) is smaller than C (%d)", ld, C);
+  SN_CHECK(ldg >= C, "smooth_l1_loss: ld of grad (%d) is smaller than C (%d)", ldg, C);
+  if (N == 0) return 0;
   smooth_l1_kernel<<<lgrid(N * C), 256, 0, (cudaStream_t)stream>>>(pred, ld, target, weight, N, C, grad_scale, grad,
                                                                  ldg, loss_sum);
   SN_LAUNCH_CHECK();

@@ -341,10 +341,17 @@ def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, spl
 # ---------------------------------------------------------------------------------------------
 # HBM-bound layers ([M, C] views of NHWC tensors; `ld` = row stride in elements)
 # ---------------------------------------------------------------------------------------------
+def _vec_aligned(t):
+    """first element on a 4-channel boundary of its storage type (16 bytes fp32, 8 bytes bf16): the least any row kernel
+    needs; the entry points check the rest (16 bytes for the row-blocked kernels, row strides)."""
+    return t.data_ptr() % (4 * t.element_size()) == 0
+
+
 def _rows(t):
     """(M, C, ld) of a tensor whose last dim is contiguous and whose leading dims collapse to rows."""
     C = t.shape[-1]
     assert t.stride(-1) == 1
+    assert not t.is_cuda or _vec_aligned(t), "row kernels read whole 4-channel vectors: misaligned channel slice"
     ld = t.stride(-2) if t.dim() >= 2 else C
     M = t.numel() // C
     return M, C, ld
