@@ -76,6 +76,9 @@ SIGNATURES = {
     "sniper_cpu_nms": ("i", "ppidp"),
     "sniper_cpu_soft_nms": ("i", "pifffu"),
     "sniper_bbox_overlaps": ("i", "pipipi"),
+    "sniper_coco_box_iou_batched": ("i", "ppppppppp" "i" "pp"),
+    "sniper_coco_match": ("i", "ppppppppppp" "i" "pi" "pi" "pppppp"),
+    "sniper_coco_accumulate": ("i", "pppppppp" "iiii" "pi" "pi" "ppp"),
 }
 
 _lib = None

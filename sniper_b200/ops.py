@@ -773,6 +773,99 @@ def proposal_nms_batched(dets, offsets):
 
 
 # ---------------------------------------------------------------------------------------------
+# COCO box evaluation (lib/dataset/pycocotools/cocoeval.py): a CSR over the non-empty (category, image) pairs; pair p
+# owns GT rows gt_off[p]:gt_off[p+1] and score-sorted detection rows dt_off[p]:dt_off[p+1] (host int32 offsets)
+# ---------------------------------------------------------------------------------------------
+def _f64(t):
+    assert t.is_cuda and t.dtype == torch.float64 and t.is_contiguous(), "expected contiguous float64 CUDA tensor"
+    return t
+
+
+def _off(off):
+    off = np.ascontiguousarray(off, dtype=np.int32)
+    assert off.ndim == 1 and off.size >= 1
+    return off
+
+
+def coco_box_iou_batched(dt_box, gt_box, gt_flags, dt_off, gt_off):
+    """bbIou (maskApi.c:98-109) of every pair: returns (ious, iou_off) with pair p's [D_p, G_p] matrix (row d = the
+    d-th detection) at ious[iou_off[p]:iou_off[p+1]] (device float64, host int64 offsets)."""
+    dt_off, gt_off = _off(dt_off), _off(gt_off)
+    P = dt_off.size - 1
+    dev = dt_box.device
+    iou_off = np.concatenate([[0], np.cumsum(np.diff(dt_off).astype(np.int64) * np.diff(gt_off))]).astype(np.int64)
+    out = torch.empty(max(int(iou_off[-1]), 1), dtype=torch.float64, device=dev)
+    d_dt, d_gt, d_iou = (torch.from_numpy(o).to(dev) for o in (dt_off, gt_off, iou_off))
+    check(lib().sniper_coco_box_iou_batched(_ptr(_f64(dt_box)), _ptr(_f64(gt_box)), _ptr(gt_flags), _ptr(d_dt),
+                                            _ptr(d_gt), _ptr(d_iou), dt_off.ctypes.data, gt_off.ctypes.data,
+                                            iou_off.ctypes.data, P, _ptr(out), _stream()))
+    return out, iou_off
+
+
+def coco_match(dt_box, dt_area, dt_id, gt_box, gt_area, gt_flags, gt_id, dt_off, gt_off, iou_thrs, area_rng,
+               full=False):
+    """evaluateImg (cocoeval.py:189-272) of every pair x area range x IoU threshold in one launch.  gt_flags uint8:
+    bit 0 iscrowd, bit 1 the annotation's `ignore`; ids int64.  Returns a dict of device tensors: dt_flags [A, T, Dtot]
+    uint8 (bit 0 matched, bit 1 ignored), npig [P, A] int32, gt_match [A, T, Gtot] int64 (matching dt id in the
+    ignore-sorted GT order), and with full=True also dt_match [A, T, Dtot] (matched gt id) and gt_order [A, Gtot]
+    (pair-local GT index at each ignore-sorted position)."""
+    dt_off, gt_off = _off(dt_off), _off(gt_off)
+    P = dt_off.size - 1
+    thr = np.ascontiguousarray(iou_thrs, dtype=np.float64)
+    rng = np.ascontiguousarray(area_rng, dtype=np.float64).reshape(-1)
+    T, A = thr.size, rng.size // 2
+    Dtot, Gtot = int(dt_off[-1]), int(gt_off[-1])
+    dev = dt_box.device
+    assert gt_flags.dtype == torch.uint8 and dt_id.dtype == torch.int64 and gt_id.dtype == torch.int64
+    r = dict(dt_flags=torch.empty(A, T, Dtot, dtype=torch.uint8, device=dev),
+             npig=torch.empty(max(P, 1), A, dtype=torch.int32, device=dev),
+             gt_match=torch.empty(A, T, Gtot, dtype=torch.int64, device=dev))
+    if full:
+        r.update(dt_match=torch.empty(A, T, Dtot, dtype=torch.int64, device=dev),
+                 gt_order=torch.empty(A, Gtot, dtype=torch.int32, device=dev))
+    d_dt, d_gt = torch.from_numpy(dt_off).to(dev), torch.from_numpy(gt_off).to(dev)
+    check(lib().sniper_coco_match(_ptr(_f64(dt_box)), _ptr(_f64(dt_area)), _ptr(dt_id), _ptr(_f64(gt_box)),
+                                  _ptr(_f64(gt_area)), _ptr(gt_flags), _ptr(gt_id), _ptr(d_dt), _ptr(d_gt),
+                                  dt_off.ctypes.data, gt_off.ctypes.data, P, thr.ctypes.data, T, rng.ctypes.data, A,
+                                  _ptr(r["dt_flags"]), _ptr(r["npig"]), _ptr(r["gt_match"]), _ptr(r.get("dt_match")),
+                                  _ptr(r.get("gt_order")), _stream()))
+    return r
+
+
+def coco_category_order(dt_score, dt_cat):
+    """The stable order of the detections by (category, descending score): cocoeval's
+    np.argsort(-dtScores, kind='mergesort') over each category's concatenation (cocoeval.py:321-325), for all categories
+    at once.  -0.0 counts as +0.0; NaN scores are refused."""
+    s = _f64(dt_score) + 0.0
+    if bool(torch.isnan(s).any()):
+        raise ValueError("coco_category_order: a detection score is NaN")
+    o1 = torch.sort(s, descending=True, stable=True).indices
+    o2 = torch.sort(dt_cat[o1], stable=True).indices
+    return o1[o2].to(torch.int32).contiguous()
+
+
+def coco_accumulate(dt_flags, dt_rank, cat_order, dt_off, npig, cat_pair_off, max_dets, rec_thrs):
+    """accumulate (cocoeval.py:274-374): precision [T, R, K, A, M] and recall [T, K, A, M] float64 (device), from
+    coco_match's dt_flags / npig, each detection's rank in its pair (dt_rank int32), coco_category_order's cat_order,
+    and cat_pair_off (host int32 [K+1]: the pairs of category k are cat_pair_off[k]:cat_pair_off[k+1])."""
+    dt_off, cat_pair_off = _off(dt_off), _off(cat_pair_off)
+    K, P = cat_pair_off.size - 1, dt_off.size - 1
+    A, T = dt_flags.shape[0], dt_flags.shape[1]
+    md = np.ascontiguousarray(max_dets, dtype=np.int32)
+    rt = np.ascontiguousarray(rec_thrs, dtype=np.float64)
+    M, R = md.size, rt.size
+    dev = dt_flags.device
+    precision = torch.empty(T, R, K, A, M, dtype=torch.float64, device=dev)
+    recall = torch.empty(T, K, A, M, dtype=torch.float64, device=dev)
+    d_dt, d_cat = torch.from_numpy(dt_off).to(dev), torch.from_numpy(cat_pair_off).to(dev)
+    check(lib().sniper_coco_accumulate(_ptr(dt_flags), _ptr(dt_rank), _ptr(cat_order), _ptr(d_dt), _ptr(npig),
+                                       _ptr(d_cat), dt_off.ctypes.data, cat_pair_off.ctypes.data, K, P, A, T,
+                                       md.ctypes.data, M, rt.ctypes.data, R, _ptr(precision), _ptr(recall),
+                                       _stream()))
+    return precision, recall
+
+
+# ---------------------------------------------------------------------------------------------
 # MobileNetV2 layers (symbols/faster/mobilenetv2_e2e.py): depthwise 3x3, first-layer im2col, shortcut add
 # ---------------------------------------------------------------------------------------------
 def depthwise3x3(x, w, stride=1, out=None):

@@ -332,11 +332,14 @@ class Tester(object):
                                    device=str(self.net.device) if self.net is not None else "cuda")
 
 
-def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device"):
-    """The CONCURRENT_JOBS == 1 path of imdb_detection_wrapper (:436-528) without the dataset evaluation: every scale of
-    TEST.SCALES in turn (FocusChips of scale i feed scale i + 1 when DO_PRUNING[i + 1]), then the cross-scale aggregation.
+def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device",
+                           imdb=None):
+    """The CONCURRENT_JOBS == 1 path of imdb_detection_wrapper (:436-528): every scale of TEST.SCALES in turn (FocusChips
+    of scale i feed scale i + 1 when DO_PRUNING[i + 1]), then the cross-scale aggregation.
     Returns (all_boxes[class][image], stats) with per-scale chip counts / detect / post-processing seconds, the NMS
-    latency and the pixel fraction processed."""
+    latency and the pixel fraction processed.  With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
+    dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
+    and its seconds to stats['eval_s']."""
     T = config.TEST
     for r in roidb:
         r['inference_crops'] = np.array([[0, 0, r['width'], r['height']]])
@@ -361,6 +364,10 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     all_boxes = tester.aggregate(detections, backend=nms_backend)
     torch.cuda.synchronize()
     stats['nms_s'] = time.time() - t0
+    if imdb is not None:
+        t0 = time.time()
+        stats['eval'] = imdb.evaluate_detections(all_boxes)
+        stats['eval_s'] = time.time() - t0
     return all_boxes, stats
 
 

@@ -67,7 +67,10 @@ DOC = {
     "sniper_cpu_nms": "cpu_nms (lib/nms/cpu_nms.pyx:112-163), host.",
     "sniper_cpu_soft_nms": "cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110), host, in place.",
     "sniper_bbox_overlaps": "bbox_overlaps_cython / ignore_overlaps_cython (lib/bbox/bbox.pyx:17-95), host, float64.",
-    "sniper_nms_gpu": "Batched hard NMS on device for per-scale inference NMS (lib/nms/nms_kernel.cu:34-144 replacement).",
+    "sniper_coco_box_iou_batched": "bbIou (lib/dataset/pycocotools/maskApi.c:98-109, reached through mask.iou from COCOeval.computeIoU, cocoeval.py:163-187) for every (category, image) pair of a CSR in ONE launch: pair p's [D_p x G_p] float64 matrix at out + iou_off[p]; crowd GTs (gt_flags bit 0) take the detection's area as the union.  Bit-exact (no FMA).",
+    "sniper_coco_match": "COCOeval.evaluateImg (lib/dataset/pycocotools/cocoeval.py:189-272) for every pair x area range x IoU threshold in ONE launch: GTs ignore-sorted (stable), min(t, 1-1e-10), crowd re-matching, the stop at the first ignored GT, ties to the later GT, ids (not booleans) as the matched test.  Writes dt_flags[A,T,Dtot] (bit 0 matched, bit 1 ignored), npig[P,A] and gt_match[A,T,Gtot] (matching dt id, 0 = none, in ignore-sorted order); dt_match[A,T,Dtot] (matched gt id) and gt_order[A,Gtot] (ignore-sorted GT order) only when non-null.",
+    "sniper_coco_accumulate": "COCOeval.accumulate (lib/dataset/pycocotools/cocoeval.py:274-374): precision[T,R,K,A,M] and recall[T,K,A,M] float64, one block per (category, area, maxDet, threshold), from sniper_coco_match's flags and one stable (category, descending score) order of the detections (cat_order) with their in-image ranks (dt_rank).  Byte-equal to the reference, -1 where it leaves -1.",
+    "sniper_nms_gpu":"Batched hard NMS on device for per-scale inference NMS (lib/nms/nms_kernel.cu:34-144 replacement).",
 }
 
 
