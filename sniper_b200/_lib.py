@@ -69,6 +69,8 @@ SIGNATURES = {
     "sniper_focus_acc": ("i", "pipl" "pp"),
     "sniper_soft_nms_batched": ("i", "ppifffuppp"),
     "sniper_proposal_nms_batched": ("i", "pppippp"),
+    "sniper_detect_post_workspace_bytes": ("z", ""),
+    "sniper_detect_post": ("i", "ppplpp" "iii" "fi" "ppll" "pp" "p"),
     "sniper_chip_input": ("i", "ppppiip"),
     "sniper_chip_input_hw": ("i", "ppppiiip"),
     "sniper_anchor_subsample": ("i", "pppiiiiiiup"),
@@ -87,7 +89,7 @@ _lib = None
 KERNELS_PER_CALL = {
     "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
-    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
+    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
 }
 launches = [0]

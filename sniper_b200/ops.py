@@ -772,6 +772,33 @@ def proposal_nms_batched(dets, offsets):
     return keep.cpu().numpy(), counts
 
 
+def detect_post_workspace(device):
+    """The scratch `detect_post` needs (block counts of one launch); reusable by launches on the same stream."""
+    return torch.empty(lib().sniper_detect_post_workspace_bytes() // 4, dtype=torch.int32, device=device)
+
+
+def detect_post(rois, cls_prob, bbox_pred, im_info, chips, rows, keys, state, workspace, *, cls_thresh=1e-3, scale=0,
+                rows_bound=0):
+    """Tester.detect's box decoding, the score threshold / chip-border pruning of get_detections and the valid-range
+    filter of aggregate (lib/inference.py:100-139, 232-351, 152-230) for one batch in one launch, no copy to the host.
+    rois [B*R,5], cls_prob [B*R,K], bbox_pred [B*R,4] (any row stride: the view the R-FCN head returns), im_info
+    [B,3]; chips: float64 [B,12] device table (`inference.chip_table`).  Surviving rows are appended to rows [cap,5] /
+    keys [cap] (int64, `inference.pack_key`) at state[0] (int64 [2]: cursor, rows a refused launch needed).
+    rows_bound: the caller's upper bound on the cursor; raises when rows_bound + B*R*(K-1) does not fit."""
+    _f32(rois), _f32(cls_prob), _f32(im_info), _f32(rows)
+    assert bbox_pred.is_cuda and bbox_pred.dtype == torch.float32 and bbox_pred.dim() == 2 and bbox_pred.shape[1] == 4 \
+        and bbox_pred.stride(1) == 1, "bbox_pred: fp32 CUDA [N,4] with unit column stride"
+    B, (N, K) = im_info.shape[0], cls_prob.shape
+    assert B > 0 and N % B == 0 and rois.shape == (N, 5) and bbox_pred.shape[0] == N
+    assert chips.is_cuda and chips.dtype == torch.float64 and chips.shape == (B, 12) and chips.is_contiguous()
+    assert keys.is_cuda and keys.dtype == torch.int64 and keys.is_contiguous() and keys.numel() == rows.shape[0]
+    assert rows.dim() == 2 and rows.shape[1] == 5 and state.is_cuda and state.dtype == torch.int64 and state.numel() == 2
+    assert workspace.is_cuda and workspace.dtype == torch.int32
+    check(lib().sniper_detect_post(_ptr(rois), _ptr(cls_prob), _ptr(bbox_pred), bbox_pred.stride(0), _ptr(im_info),
+                                   _ptr(chips), B, N // B, K, float(cls_thresh), int(scale), _ptr(rows), _ptr(keys),
+                                   rows.shape[0], int(rows_bound), _ptr(state), _ptr(workspace), _stream()))
+
+
 # ---------------------------------------------------------------------------------------------
 # COCO box evaluation (lib/dataset/pycocotools/cocoeval.py): a CSR over the non-empty (category, image) pairs; pair p
 # owns GT rows gt_off[p]:gt_off[p+1] and score-sorted detection rows dt_off[p]:dt_off[p+1] (host int32 offsets)

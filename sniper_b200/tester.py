@@ -8,7 +8,10 @@ Host-side mirror of `lib/iterators/MNIteratorTestAutoFocus.py` (:13-141), `lib/i
   reference                                             here
   cv2 crop / resize / pad in a thread pool              one `sniper_chip_input_hw` launch per batch (uint8 crops over PCIe)
   MXNet module forward (RPN, MultiProposal op on host)  `SniperResNet101.forward_inference` (device MultiProposal)
-  bbox_pred / clip / rescale in numpy per chip          the same numpy code (`inference.detect_postprocess`)
+  bbox_pred / clip / rescale in numpy per chip          the same numpy code (`inference.detect_postprocess`), or with
+                                                        backend="device" one `sniper_detect_post` launch per batch into
+                                                        a device run buffer (no detection crosses to the host before
+                                                        the soft-NMS has run)
   per-(image, class) cpu_soft_nms in a Pool(32)         ONE `sniper_soft_nms_batched` launch for the whole run
   FocusChips with OpenCV                                `chips_inference.add_chips`
 
@@ -298,8 +301,14 @@ class Tester(object):
         return scores, preds, batch, batch['im_ids'], maps, batch['chip_ids']
 
     def get_detections(self, cls_thresh=1e-3, cache_name='cache', evaluate=False, vis=False, vis_path=None,
-                       do_pruning=False, autofocus=False, vis_ext='.png'):
-        """(all_boxes, all_maps) (:232-370): all_boxes[j][im][chip] = [n,5], all_maps[im][chip] = (None, FocusPixel map)."""
+                       do_pruning=False, autofocus=False, vis_ext='.png', backend="host", scale_index=0):
+        """(all_boxes, all_maps) (:232-370): all_boxes[j][im][chip] = [n,5], all_maps[im][chip] = (None, FocusPixel map).
+        backend="device": all_boxes is the scale's `inference.DeviceDetections` instead (rows already through
+        TEST.VALID_RANGES[scale_index]); see `_get_detections_device`."""
+        if backend == "device":
+            return self._get_detections_device(cls_thresh, do_pruning, autofocus, scale_index)
+        if backend != "host":
+            raise ValueError("get_detections: backend must be 'host' or 'device', not %r" % (backend,))
         n_chips = [len(r['inference_crops']) for r in self.roidb]
         all_boxes = [[[np.zeros((0, 5), np.float32) for _ in range(n_chips[i])] for i in range(self.num_images)]
                      for _ in range(self.num_classes)]
@@ -323,6 +332,38 @@ class Tester(object):
             self.post_time += time.time() - t0
         return all_boxes, all_maps
 
+    def _get_detections_device(self, cls_thresh, do_pruning, autofocus, scale_index):
+        """The batches of the scale with the detections kept on the device: `forward_inference`, then `ops.detect_post`
+        on its output tensors, fed by the batch's chip table.  Only the FocusPixel maps come to the host (FocusChips are
+        generated there), by non-blocking copies into pinned memory that are waited for once, after the last batch."""
+        want_map = bool(getattr(self.cfg.TEST, "AUTO_FOCUS", False)) and self.net.af is not None
+        dets = inference.DeviceDetections(self.net.device)
+        all_maps = [[[] for _ in r['inference_crops']] for r in self.roidb]
+        seen, staged = set(), []
+        t0 = time.time()
+        for batch in self.test_iter:
+            out = self.net.forward_inference(batch['data'], batch['im_info'], autofocus=want_map)
+            rois, _, cls_prob, deltas = out[:4]
+            table = inference.chip_table(self.roidb, batch['im_ids'], batch['chip_ids'], do_pruning,
+                                         self.cfg.TEST.VALID_RANGES[scale_index], seen)
+            dets.append(rois, cls_prob, deltas, batch['im_info'], table, cls_thresh=cls_thresh, scale=scale_index)
+            if want_map and autofocus:
+                fm = torch.empty(out[4].shape, dtype=out[4].dtype, pin_memory=True)
+                info = torch.empty(batch['im_info'].shape, dtype=torch.float32, pin_memory=True)
+                fm.copy_(out[4], non_blocking=True)
+                info.copy_(batch['im_info'], non_blocking=True)
+                staged.append((fm, info, batch['im_ids'], batch['chip_ids']))
+        dets.finish()
+        self.detect_time += time.time() - t0
+        t0 = time.time()
+        for fm, info, im_ids, chip_ids in staged:
+            fm, info = fm.numpy(), info.numpy()
+            for idx, (im_id, chip_id) in enumerate(zip(im_ids, chip_ids)):
+                mh, mw = int(math.ceil(info[idx, 0] / 16.0)), int(math.ceil(info[idx, 1] / 16.0))
+                all_maps[im_id][chip_id] = (None, fm[idx, :mh, :mw].copy())
+        self.post_time += time.time() - t0
+        return dets, all_maps
+
     def aggregate(self, scale_cls_dets, vis=False, cache_name='cache', vis_path=None, vis_name=None, pre_nms_db_divide=10,
                   vis_ext='.png', backend="device"):
         t = self.cfg.TEST
@@ -333,11 +374,13 @@ class Tester(object):
 
 
 def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device",
-                           imdb=None):
+                           imdb=None, detect_backend="host"):
     """The CONCURRENT_JOBS == 1 path of imdb_detection_wrapper (:436-528): every scale of TEST.SCALES in turn (FocusChips
     of scale i feed scale i + 1 when DO_PRUNING[i + 1]), then the cross-scale aggregation.
     Returns (all_boxes[class][image], stats) with per-scale chip counts / detect / post-processing seconds, the NMS
-    latency and the pixel fraction processed.  With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
+    latency and the pixel fraction processed.  detect_backend="device" keeps the detections on the GPU from the network
+    to the soft-NMS (`Tester.get_detections(backend="device")`); stats then carry `detections_pre_nms` per scale.
+    With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
     dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
     and its seconds to stats['eval_s']."""
     T = config.TEST
@@ -349,9 +392,12 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
         it = MNIteratorTestAutoFocus(roidb, config, scale, batch_size=nbatch, device=device)
         tester = Tester(net, None, roidb, it, config, batch_size=nbatch, num_classes=num_classes)
         t0 = time.time()
-        dets, maps = tester.get_detections(do_pruning=bool(T.DO_PRUNING[scale_i]), autofocus=bool(T.AUTO_FOCUS))
+        dets, maps = tester.get_detections(do_pruning=bool(T.DO_PRUNING[scale_i]), autofocus=bool(T.AUTO_FOCUS),
+                                           backend=detect_backend, scale_index=scale_i)
         st = dict(scale=tuple(scale), chips=int(it.n_chips), batches=int(it.size // max(nbatch, 1)),
                   detect_s=tester.detect_time, post_s=tester.post_time, total_s=time.time() - t0)
+        if detect_backend == "device":
+            st['detections_pre_nms'] = len(dets)
         if scale_i + 1 < len(T.SCALES) and T.DO_PRUNING[scale_i + 1] and T.AUTO_FOCUS:
             t1 = time.time()
             area = chips_inference.add_chips(roidb, maps, scale_i, config)
