@@ -81,6 +81,8 @@ SIGNATURES = {
     "sniper_coco_box_iou_batched": ("i", "ppppppppp" "i" "pp"),
     "sniper_coco_match": ("i", "ppppppppppp" "i" "pi" "pi" "pppppp"),
     "sniper_coco_accumulate": ("i", "pppppppp" "iiii" "pi" "pi" "ppp"),
+    "sniper_train_metric_workspace_bytes": ("z", ""),
+    "sniper_train_metric_accum": ("i", "pipiiii" "pipii" "pipii" "ppppp"),
 }
 
 _lib = None
@@ -89,7 +91,7 @@ _lib = None
 KERNELS_PER_CALL = {
     "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
-    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
+    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
 }
 launches = [0]

@@ -16,6 +16,7 @@ bbox_pred (4 rows); output rows are zero-padded to the tile-friendly counts the 
 import struct
 
 import numpy as np
+import torch
 
 LIST_MAGIC = 0x112
 V1_MAGIC = 0xF993FAC8
@@ -64,8 +65,8 @@ def _read_ndarray(r):
     return np.frombuffer(r.raw(n * dt.itemsize), dtype=dt).reshape(shape).copy()
 
 
-def read_params(path):
-    """`mx.nd.load` + the arg:/aux: split of load_checkpoint (utils.py:56-65) -> (arg_params, aux_params) as numpy."""
+def read_list(path):
+    """`mx.nd.load` of a named NDArray list -> [(name, numpy array)] in file order."""
     r = _Reader(open(path, "rb").read())
     if r.take("Q") != LIST_MAGIC:
         raise ValueError("%s is not an MXNet NDArray list file" % path)
@@ -74,8 +75,13 @@ def read_params(path):
     names = [r.raw(r.take("Q")).decode() for _ in range(r.take("Q"))]
     if len(names) != len(arrays):
         raise ValueError("unnamed NDArray lists are not checkpoints")
+    return list(zip(names, arrays))
+
+
+def read_params(path):
+    """`mx.nd.load` + the arg:/aux: split of load_checkpoint (utils.py:56-65) -> (arg_params, aux_params) as numpy."""
     arg, aux = {}, {}
-    for k, v in zip(names, arrays):
+    for k, v in read_list(path):
         tp, name = k.split(":", 1)
         (arg if tp == "arg" else aux)[name] = v
     return arg, aux
@@ -83,7 +89,11 @@ def read_params(path):
 
 def write_params(path, arg, aux):
     """`mx.model.save_checkpoint`'s `.params` half (NDArray v2, dense, cpu context)."""
-    items = [("arg:" + k, v) for k, v in arg.items()] + [("aux:" + k, v) for k, v in aux.items()]
+    write_list(path, [("arg:" + k, v) for k, v in arg.items()] + [("aux:" + k, v) for k, v in aux.items()])
+
+
+def write_list(path, items):
+    """`mx.nd.save` of a named NDArray list [(name, numpy array)]."""
     out = [struct.pack("<QQQ", LIST_MAGIC, 0, len(items))]
     for _, v in items:
         v = np.ascontiguousarray(v)
@@ -212,3 +222,49 @@ def conv_to_reference(name, cout, cin, k, w_rows, b, part_rows=None, out=None):
             out[n + "_bias"] = np.ascontiguousarray(b[r0:r0 + c])
         r0 += c
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# optimizer state (`<prefix>-%04d.states`)
+# ---------------------------------------------------------------------------------------------------------------
+def _momentum_index(net):
+    """For every trainable tensor of net.export_reference(grads=True) (reference name and layout): the flat position of
+    each element in net.P.  Found by exporting an index image of the gradient buffer (two halves, each exact in float32)
+    and restoring the buffer afterwards, so the momenta go through exactly the conversions the weights go through."""
+    P = net.P
+    saved = P.g.clone()
+    idx = torch.arange(P.total, device=P.g.device)
+    parts = []
+    try:
+        for v in (idx % 4096, idx // 4096):
+            P.g.copy_(v.float())
+            parts.append(net.export_reference(grads=True)[0])
+    finally:
+        P.g.copy_(saved)
+    return {k: parts[0][k].astype(np.int64) + 4096 * parts[1][k].astype(np.int64) for k in parts[0]}
+
+
+def save_optimizer_states(path, net, num_update):
+    """The SGD state a stopped run needs: the momentum of every trainable tensor as `mom:<reference name>` in the
+    reference's layout, and the update count as int64 `num_update`, in the NDArray-list format of `.params` files.
+    (MXNet's own `.states` is a pickled Updater.states dict, optimizer.py:1487-1505: the two are not interchangeable.)"""
+    mom = net.P.mom.detach().cpu().numpy()
+    items = [("mom:" + k, np.ascontiguousarray(mom[v])) for k, v in _momentum_index(net).items()]
+    items.append(("num_update", np.array([int(num_update)], dtype=np.int64)))
+    write_list(path, items)
+    return path
+
+
+def load_optimizer_states(path, net):
+    """Inverse of save_optimizer_states: fills net.P.mom and returns num_update."""
+    items = dict(read_list(path))
+    mom = np.zeros(net.P.total, dtype=np.float32)
+    for k, v in _momentum_index(net).items():
+        m = items.get("mom:" + k)
+        if m is None or m.shape != v.shape:
+            raise ValueError("%s: no momentum of shape %s for %s" % (path, v.shape, k))
+        mom[v] = m
+    if "num_update" not in items:
+        raise ValueError("%s has no num_update" % path)
+    net.P.mom.copy_(torch.from_numpy(mom))
+    return int(items["num_update"].reshape(-1)[0])

@@ -89,7 +89,13 @@ def chip_ground_truth(im_info, cur_crop, im_scale, nids, gtids, gt_boxes, boxes,
 
 
 class RawBatch(object):
-    """Pinned host buffers of one batch (what crosses PCIe): source pixels + small per-chip arrays."""
+    """Pinned host buffers of one batch (what crosses PCIe): source pixels + small per-chip arrays.
+
+    MNIteratorE2E reuses a ring of `n_buffers` of these.  InputStage.run copies a batch to the device with
+    asynchronous H2D copies, so a buffer may be refilled only after the step that read it has completed.  A caller
+    that synchronises every step (Trainer.step_raw) needs depth + 2 buffers behind a PrefetchingIter of that depth;
+    Trainer.fit keeps the host at most one step ahead (it waits for step i-1 before it takes batch i+1), so two
+    batches can be in flight and it needs depth + 3."""
 
     def __init__(self, B, max_gt, pixel_capacity, focus_cap=0):
         """focus_cap > 0 (TRAIN.AUTO_FOCUS): room for that many FocusPixel boxes per chip (`focus_boxes`, `nfocus`)."""
@@ -299,17 +305,22 @@ class MNIteratorE2E(object):
         return raw
 
 
+EPOCH_END = object()      # what PrefetchingIter(epoch_marker=True) yields after the last batch of every epoch
+
+
 class PrefetchingIter(object):
     """Background-thread prefetch of raw batches (the role of mx.io.PrefetchingIter around MNIteratorE2E in
     main_train.py): the host bookkeeping of batch i+1 runs while the GPU computes batch i.  The wrapped iterator must
-    own at least depth + 2 raw buffers (n_buffers)."""
+    own at least depth + 2 raw buffers (n_buffers; depth + 3 under Trainer.fit, see RawBatch).  Epochs follow each
+    other silently unless epoch_marker=True, which yields `EPOCH_END` after each one."""
 
-    def __init__(self, it, depth=2, epochs=None):
+    def __init__(self, it, depth=2, epochs=None, epoch_marker=False):
         import queue
         import threading
         self.it = it
         self.q = queue.Queue(maxsize=depth)
         self.epochs = epochs
+        self.epoch_marker = epoch_marker
         self._stop = False
         # Every ctypes call of the training step releases the GIL and has to win it back from the producer thread; with
         # the default 5 ms switch interval each of those hand-overs can stall the step by up to 5 ms (measured: step_raw
@@ -327,6 +338,8 @@ class PrefetchingIter(object):
                 if self._stop:
                     return
                 self.q.put(raw)
+            if self.epoch_marker:
+                self.q.put(EPOCH_END)
             ep += 1
             if self.epochs is not None and ep >= self.epochs:
                 self.q.put(None)
@@ -446,13 +459,22 @@ def synthetic_roidb(n_images, seed=0, width=1333, height=800, n_gt=(1, 20), n_pr
     return out
 
 
-def default_config(neg=True, autofocus=False):
+def default_config(neg=True, autofocus=False, network="resnet101"):
     """The slice of configs/faster/sniper_res101_e2e.yml the iterator reads (:21-39, 76-101, 120-140); autofocus=True:
-    TRAIN.AUTO_FOCUS of configs/faster/sniper_res101_e2e_autofocus.yml (FocusPixel labels, thresholds 5 / 64 / 90)."""
+    TRAIN.AUTO_FOCUS of configs/faster/sniper_res101_e2e_autofocus.yml (FocusPixel labels, thresholds 5 / 64 / 90).
+    network="mobilenetv2": the network block of configs/faster/sniper_mobilenetv2_e2e.yml instead (stride 32, scales
+    1 / 2 / 4 / 8 / 12: 15 anchors), for model_mnv2.SniperMobileNetV2."""
     import types
     S = types.SimpleNamespace
-    return S(network=S(PIXEL_MEANS=[103.06, 115.90, 123.15], ANCHOR_SCALES=[2, 4, 7, 10, 13, 16, 24],
-                       ANCHOR_RATIOS=[0.5, 1, 2], RPN_FEAT_STRIDE=16, NUM_ANCHORS=21),
+    if network == "resnet101":
+        net = S(PIXEL_MEANS=[103.06, 115.90, 123.15], ANCHOR_SCALES=[2, 4, 7, 10, 13, 16, 24], ANCHOR_RATIOS=[0.5, 1, 2],
+                RPN_FEAT_STRIDE=16, NUM_ANCHORS=21)
+    elif network == "mobilenetv2":
+        net = S(PIXEL_MEANS=[103.939, 116.779, 123.68], ANCHOR_SCALES=[1, 2, 4, 8, 12], ANCHOR_RATIOS=[0.5, 1, 2],
+                RPN_FEAT_STRIDE=32, NUM_ANCHORS=15)
+    else:
+        raise ValueError("default_config: network must be 'resnet101' or 'mobilenetv2', not %r" % (network,))
+    return S(network=net,
              TRAIN=S(SCALES=[(1400, 2000), (800, 1280), (-1, 512)], VALID_RANGES=[(-1, 80), (32, 150), (120, -1)],
                      CPP_CHIPS=True, USE_NEG_CHIPS=neg, RPN_BATCH_SIZE=256, RPN_FG_FRACTION=0.5,
                      RPN_POSITIVE_OVERLAP=0.5, RPN_NEGATIVE_OVERLAP=0.4, BATCH_IMAGES=16, AUTO_FOCUS=autofocus,

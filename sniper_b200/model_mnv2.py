@@ -164,6 +164,9 @@ class SniperMobileNetV2:
     """mobilenetv2_e2e.get_symbol_rcnn(cfg, is_train=True) as an executable object."""
 
     n_phases = 1
+    # the R-CNN loss is not normalised by the valid count (:281-282), so cnt_buf[1] stays 0: the trainer's metric
+    # launch counts the rows itself
+    rcnn_valid_counted = False
 
     def __init__(self, cfg=None, device="cuda", seed=5):
         self.cfg = cfg or MCfg()

@@ -736,6 +736,29 @@ def focus_acc(prob, label, counts):
     check(lib().sniper_focus_acc(_ptr(prob), prob.stride(-2), _ptr(label), n, _ptr(counts), _stream()))
 
 
+def train_metric_workspace(device):
+    """The zero-filled scratch sniper_train_metric_accum needs (reusable across launches and graph replays)."""
+    return torch.zeros(int(lib().sniper_train_metric_workspace_bytes()), dtype=torch.uint8, device=device)
+
+
+def train_metric_accum(rpn_prob, rpn_label, A, cls_prob, cls_label, counts, loss_buf, acc, workspace, af_prob=None,
+                       af_label=None):
+    """Adds one step's training-metric terms into `acc` (int64 [24]: num_inst[8] | hits[8] | float64 sum[8], see
+    csrc/train_metric.cu).  rpn_prob NHWC [B,H,W,>=2A], rpn_label [B,A*H*W]; cls_prob [N,>=K] (K = its width),
+    cls_label [N]; af_prob [B,Hf,Wf,>=2] / af_label [B,Hf*Wf] or None; counts int32 (count_valid results), loss_buf
+    the step's loss sums."""
+    B, H, W, _ = rpn_prob.shape
+    N, K = cls_prob.shape
+    assert acc.dtype == torch.int64 and acc.numel() == 24 and acc.is_contiguous() and counts.dtype == torch.int32
+    Haf = Waf = ld_af = 0
+    if af_prob is not None:
+        Haf, Waf, ld_af = af_prob.shape[1], af_prob.shape[2], af_prob.stride(2)
+    check(lib().sniper_train_metric_accum(_ptr(rpn_prob), rpn_prob.stride(2), _ptr(rpn_label), B, H, W, int(A),
+                                          _ptr(cls_prob), cls_prob.stride(0), _ptr(cls_label), N, K,
+                                          _ptr(af_prob), ld_af, _ptr(af_label), Haf, Waf,
+                                          _ptr(counts), _ptr(loss_buf), _ptr(acc), _ptr(workspace), _stream()))
+
+
 def soft_nms_batched(dets, offsets, *, sigma=0.55, Nt=0.3, threshold=0.001, method=2):
     """cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110) on every segment dets[offsets[p]:offsets[p+1]] ([.,5] rows x1,y1,x2,y2,score)
     at once.  Returns (dets_out, counts): the first counts[p] rows of segment p are its surviving detections in the

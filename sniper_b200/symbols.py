@@ -298,6 +298,7 @@ def bind_graph(sym, device="cuda:0", **overrides):
     net = ours.bind(device, **kw)
     if info["autofocus"] and not af_train:
         net.enable_autofocus()
+    net.symbol = sym            # written next to the checkpoints as `<prefix>-symbol.json`
     return net
 
 

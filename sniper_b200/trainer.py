@@ -7,19 +7,31 @@ forward+backward, ONE NCCL all-reduce over the flat gradient bucket (replaces th
 push/pull, model.py:126-136 / comm.h:433-553; sum without 1/N as rescale_grad=1.0, utils.py:30,37), one
 CUDA-graph replay of the fused SGD-momentum update, D2H of the four loss scalars (what the reference's
 metrics read with asnumpy(), lib/train_utils/metric.py:109-125).
+
+`fit` is BaseModule.fit's epoch loop (base_module.py:500-550) on top of that step.  It turns on the device metrics
+(`metrics=True`): one `sniper_train_metric_accum` launch per step, after the update, accumulates the reference's
+training metrics on the device, so a step needs no host synchronisation and the metrics are read only when printed.
 """
+import logging
+import time
+from collections import namedtuple
+
 import torch
 
-from . import lr_scheduler, model, ops
+from . import checkpoint, lr_scheduler, metric, model, ops
+
+# mxnet.model.BatchEndParam (SNIPER-mxnet/python/mxnet/model.py:51-56)
+BatchEndParam = namedtuple("BatchEndParams", ["epoch", "nbatch", "eval_metric", "locals"])
 
 
 class Trainer:
     def __init__(self, cfg=None, device="cuda:0", world_size=1, use_graph=True, seed=5, deform_offset_std=0.0,
-                 scheduler="config", net=None):
+                 scheduler="config", net=None, metrics=False):
         """scheduler: "config" = the reference's WarmupMultiBatchScheduler built from cfg (lr, lr_step, warmup*), None =
         constant cfg.lr, or any callable num_update -> lr.  net: an already constructed network exposing the same
         surface as model.SniperResNet101 (P, fb_phases, forward_backward, train_bns, set_lr, update), e.g.
-        model_mnv2.SniperMobileNetV2; default: the ResNet-101 graph built from cfg."""
+        model_mnv2.SniperMobileNetV2; default: the ResNet-101 graph built from cfg.  metrics: accumulate the training
+        metrics on the device after every step (`metric_acc`; `fit` turns this on)."""
         self.cfg = cfg or (net.cfg if net is not None else model.Cfg())
         self.device = torch.device(device)
         torch.cuda.set_device(self.device)
@@ -53,6 +65,38 @@ class Trainer:
                                                  batch_size=getattr(c, "batch_images", 16) * world_size)
         self.scheduler = scheduler
         self.lr = self.cfg.lr
+        self.metric_acc = None
+        self.g_metric = None
+        if metrics:
+            self.enable_metrics()
+
+    def enable_metrics(self):
+        """Adds the metric launch to every following step (and, with graphs, a small graph replayed after the update)."""
+        if self.metric_acc is None:
+            self.metric_acc = metric.MetricAccumulator(self.device, self.world_size)
+            if self.g_up is not None:
+                self._capture_metric(torch.cuda.graph_pool_handle())
+        return self.metric_acc
+
+    def _metric_launch(self, out, acc=None):
+        """The step's metric terms into the accumulator: RPN probabilities against the batch's anchor labels, R-CNN
+        class probabilities against MultiProposalTarget's labels, and (AutoFocus) the FocusPixel softmax."""
+        net = self.net
+        if not getattr(net, "rcnn_valid_counted", True):
+            ops.count_valid(out["label"], net.cnt_buf[1:2])      # a net whose R-CNN loss does not count its rows
+        ops.train_metric_accum(out["rpn_cls_prob"], self.static["label"], net.cfg.num_anchors, out["cls_prob"],
+                               out["label"], net.cnt_buf, net.loss_buf, self.metric_acc.buf if acc is None else acc,
+                               self.metric_acc.workspace, af_prob=out.get("cls_scale_prob"),
+                               af_label=out.get("scale_label"))
+
+    def _capture_metric(self, pool):
+        # one eager launch first loads the kernel outside capture; its sum goes to a scratch accumulator and is dropped
+        self._metric_launch(self.out, acc=torch.zeros_like(self.metric_acc.buf))
+        torch.cuda.synchronize()
+        self.g_metric = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.g_metric, pool=pool):
+            self._metric_launch(self.out)
+        torch.cuda.synchronize()
 
     def next_lr(self, lr=None):
         """mxnet.optimizer: `_update_count` then `_get_lr` -> scheduler(num_update) with the incremented count."""
@@ -137,6 +181,9 @@ class Trainer:
         for b, (m, v) in zip(self.net.train_bns(), snap[2]):
             b.st.moving_mean.copy_(m)
             b.st.moving_var.copy_(v)
+        # the warm-up's lr-0 updates still move the weights by the momentum (non-zero after a resume), and the bf16
+        # copies with them: rebuild those from the restored fp32 masters
+        P.sync_lowp()
 
     def capture(self):
         """Warm up eagerly, then capture forward+backward and the optimizer update as two CUDA graphs.  The warm-up runs
@@ -173,6 +220,8 @@ class Trainer:
         with torch.cuda.graph(self.g_up, pool=pool):
             self.net.update()
         torch.cuda.synchronize()
+        if self.metric_acc is not None:
+            self._capture_metric(pool)
 
     def step_device(self, lr=None):
         """One training step on the batch currently in the static buffers.  The learning rate comes from the schedule
@@ -184,16 +233,23 @@ class Trainer:
                 self._allreduce_bucket(k)
             self._allreduce_finish()
             self.g_up.replay()
+            if self.g_metric is not None:
+                self.g_metric.replay()
         else:
             self.out = self.net.forward_backward(self.static, on_bucket=self._allreduce_bucket)
             self._allreduce_finish()
             self.net.update()
+            if self.metric_acc is not None:
+                self._metric_launch(self.out)
         return self.out
 
     # ---- public end-to-end step from the iterator's raw batch (uint8 source rectangles + chip tables)
     def step_raw(self, raw, input_stage, lr=None):
         """One training step on a `iterator.RawBatch`: H2D of the raw bytes, GPU input stage (resize / mean / flip,
         anchor matching, label subsampling), forward + backward + all-reduce + update, D2H of the losses."""
+        return self._losses(self._enqueue_raw(raw, input_stage, lr))
+
+    def _enqueue_raw(self, raw, input_stage, lr):
         batch = input_stage.run(raw)
         if self.static is None:
             self.static = {k: torch.empty_like(v) for k, v in batch.items()}
@@ -201,7 +257,16 @@ class Trainer:
             self.static[k].copy_(v, non_blocking=True)
         if self.g_fb is None and self.use_graph:
             self.capture()
-        return self._losses(self.step_device(lr))
+        return self.step_device(lr)
+
+    def step_raw_async(self, raw, input_stage, lr=None):
+        """step_raw without the loss read-back: enqueues the step (and, with metrics on, its metric launch) and returns
+        at once with an event that completes with the step.  The raw batch's pinned buffers are read by asynchronous
+        H2D copies until then."""
+        self._enqueue_raw(raw, input_stage, lr)
+        done = torch.cuda.Event()
+        done.record()
+        return done
 
     def _losses(self, out):
         """D2H of the step's loss buffer (one 32-byte copy) -> the metric values; an AutoFocus net adds the cls_scale_prob
@@ -227,3 +292,96 @@ class Trainer:
         if self.g_fb is None and self.use_graph:
             self.capture()
         return self._losses(self.step_device(lr))
+
+    # ---- checkpoints (Module.save_checkpoint / load_optimizer_states, module.py:160-180, 775-805)
+    def save_checkpoint(self, prefix, epoch, save_optimizer_states=False):
+        """`<prefix>-%04d.params` through checkpoint.save_checkpoint (with the `*_test` box-regression tensors), the
+        bound Symbol's `<prefix>-symbol.json` when the net came from one, and `<prefix>-%04d.states` (momenta and the
+        update count) when asked."""
+        arg, aux = self.net.export_reference()
+        sym = getattr(self.net, "symbol", None)
+        if sym is not None:
+            sym.save("%s-symbol.json" % prefix)
+        checkpoint.save_checkpoint(prefix, epoch, arg, aux)
+        if save_optimizer_states:
+            checkpoint.save_optimizer_states("%s-%04d.states" % (prefix, epoch), self.net, self.num_update)
+
+    def load_optimizer_states(self, fname):
+        """Momenta and update count of a `.states` file written by save_checkpoint: the next step continues the run
+        (the learning-rate schedule follows num_update)."""
+        self.num_update = checkpoint.load_optimizer_states(fname, self.net)
+
+    # ---- the epoch loop
+    def fit(self, train_iter, input_stage, num_epoch, begin_epoch=0, eval_metric=None, batch_end_callback=None,
+            epoch_end_callback=None):
+        """BaseModule.fit (SNIPER-mxnet/python/mxnet/module/base_module.py:500-550) over raw batches.
+
+        train_iter: an `iterator.PrefetchingIter(..., epoch_marker=True)` (an epoch ends at its marker: the chip count
+        changes from epoch to epoch with the negative-chip draw), or any iterator of raw batches that ends each epoch
+        with StopIteration and has `reset()`.  eval_metric: a `metric` object (default: main_train.py's composite);
+        it is bound to this trainer's device accumulator.  batch_end_callback(BatchEndParam) after every step,
+        epoch_end_callback(epoch, symbol, arg_params, aux_params) after every epoch; lists are accepted.
+
+        The host runs at most one step ahead of the device: before step i+1 is enqueued (and before its raw batch is
+        taken from the iterator) step i-1 has completed, so at most two raw batches are read by in-flight H2D copies.
+        With several ranks every rank must call fit; metric reads are collective, and only rank 0 logs.  Every rank's
+        iterator must yield the same number of batches per epoch (the negative-chip draw sets it, so seed the ranks'
+        draws alike): a rank whose epoch ends early leaves the others waiting in a collective.  Not run on more than
+        one GPU yet."""
+        from . import iterator
+        if isinstance(train_iter, iterator.PrefetchingIter) and not train_iter.epoch_marker:
+            raise ValueError("fit: a PrefetchingIter needs epoch_marker=True (it would run one endless epoch)")
+        if isinstance(train_iter, iterator.PrefetchingIter) and hasattr(train_iter.it, "_buffers"):
+            need = train_iter.q.maxsize + 3
+            if len(train_iter.it._buffers) < need:
+                raise ValueError("fit: the iterator owns %d raw buffers; with prefetch depth %d it needs %d (two "
+                                 "batches in flight, see iterator.RawBatch)" % (len(train_iter.it._buffers),
+                                                                                train_iter.q.maxsize, need))
+        acc = self.enable_metrics()
+        if eval_metric is None:
+            eval_metric = metric.default_metrics(bool(getattr(self.net.cfg, "autofocus", False)))
+        eval_metric.bind(acc)
+        rank0 = self.world_size == 1 or torch.distributed.get_rank() == 0
+        log = logging.getLogger()
+        as_list = lambda c: [] if c is None else (c if isinstance(c, (list, tuple)) else [c])
+        marker = getattr(iterator, "EPOCH_END", None)
+
+        def fetch(it):
+            try:
+                b = next(it)
+            except StopIteration:
+                return None
+            return None if b is marker else b
+
+        for epoch in range(begin_epoch, num_epoch):
+            tic = time.time()
+            eval_metric.reset()
+            nbatch = 0
+            it = iter(train_iter)
+            done = [None, None]                  # completion events of the last two steps enqueued
+            next_raw = fetch(it)
+            eval_name_vals = []
+            while next_raw is not None:
+                raw = next_raw
+                done = [done[1], self.step_raw_async(raw, input_stage)]
+                if done[0] is not None:
+                    done[0].synchronize()        # step i-1 done: its raw batch may be refilled
+                next_raw = fetch(it)
+                if next_raw is None:
+                    eval_name_vals = eval_metric.get_name_value()
+                param = BatchEndParam(epoch=epoch, nbatch=nbatch, eval_metric=eval_metric, locals=locals())
+                for cb in as_list(batch_end_callback):
+                    cb(param)
+                nbatch += 1
+            if done[1] is not None:
+                done[1].synchronize()
+            if rank0:
+                for name, val in eval_name_vals:
+                    log.info("Epoch[%d] Train-%s=%f", epoch, name, val)
+                log.info("Epoch[%d] Time cost=%.3f", epoch, time.time() - tic)
+            if epoch_end_callback is not None:
+                arg, aux = self.net.export_reference()
+                for cb in as_list(epoch_end_callback):
+                    cb(epoch, getattr(self.net, "symbol", None), arg, aux)
+            if not isinstance(train_iter, iterator.PrefetchingIter):
+                train_iter.reset()
