@@ -171,17 +171,50 @@ __global__ void __launch_bounds__(256) deform_im2col_kernel(DcArgs p) {
   }
 }
 
-int fill(DcArgs& a, const void* x, const float* offset, int NB, int H, int W, int C, int KH, int KW, int stride,
-         int dil, int pad, int dgroups, int off_ld) {
-  SN_CHECK(C % 128 == 0, "deform conv: C (%d) must be a multiple of 128", C);
+// floor((extent + 2 pad - dil (k - 1) - 1) / stride) + 1, or 0 when the dilated kernel does not fit once
+long out_extent(int extent, int k, int stride, int dil, int pad) {
+  const long span = (long)extent + 2L * pad - (long)dil * (k - 1) - 1;
+  return span < 0 ? 0 : span / stride + 1;
+}
+
+// Every rule the kernels rely on, checked before any CUDA call: the warps read x and write col as whole 16-byte (fp32)
+// or 8-byte (bf16) vectors of 4 channels, and the offsets as single floats.  `who` names the entry point.
+int fill(DcArgs& a, const char* who, const void* x, const float* offset, int NB, int H, int W, int C, int KH, int KW,
+         int stride, int dil, int pad, int dgroups, int off_ld, const void* col, int dtype) {
+  SN_CHECK(dtype == 0 || dtype == 1, "%s: dtype must be 0 (fp32) or 1 (bf16)", who);
+  SN_CHECK(NB >= 0 && H >= 0 && W >= 0, "%s: NB (%d), H (%d) and W (%d) must not be negative", who, NB, H, W);
+  SN_CHECK(KH >= 1 && KW >= 1, "%s: KH (%d) and KW (%d) must be at least 1", who, KH, KW);
+  SN_CHECK(stride >= 1, "%s: stride (%d) must be at least 1", who, stride);
+  SN_CHECK(dil >= 1, "%s: dil (%d) must be at least 1", who, dil);
+  SN_CHECK(pad >= 0, "%s: pad (%d) must not be negative", who, pad);
+  SN_CHECK(C > 0 && C % 128 == 0, "%s: C (%d) must be a positive multiple of 128", who, C);
   SN_CHECK(dgroups > 0 && C % dgroups == 0 && (C / dgroups) % 128 == 0,
-           "deform conv: channels per deformable group must be a multiple of 128");
-  SN_CHECK(off_ld >= dgroups * 2 * KH * KW, "deform conv: offset row stride too small");
+           "%s: channels per deformable group (C %d / dgroups %d) must be a multiple of 128", who, C, dgroups);
+  SN_CHECK(off_ld >= dgroups * 2 * KH * KW, "%s: offset row stride off_ld (%d) is smaller than 2*dgroups*KH*KW (%d)",
+           who, off_ld, dgroups * 2 * KH * KW);
+  // a batch of empty maps would size the fp64-scratch reduction to nothing: only NB == 0 is an empty call
+  SN_CHECK(NB == 0 || (H >= 1 && W >= 1), "%s: H (%d) and W (%d) must be at least 1 when NB (%d) > 0", who, H, W, NB);
+  const long Ho = out_extent(H, KH, stride, dil, pad), Wo = out_extent(W, KW, stride, dil, pad);
+  SN_CHECK(NB == 0 || (Ho >= 1 && Wo >= 1), "%s: the output map is empty (Ho %ld, Wo %ld)", who, Ho, Wo);
+  SN_CHECK(x != nullptr && offset != nullptr && col != nullptr, "%s: x / offset / col must not be null", who);
+  const uintptr_t vec = dtype == 0 ? 16 : 8;
+  SN_CHECK(((uintptr_t)x & (vec - 1)) == 0, "%s: x must be %d-byte aligned", who, (int)vec);
+  SN_CHECK(((uintptr_t)col & (vec - 1)) == 0, "%s: col must be %d-byte aligned", who, (int)vec);
+  SN_CHECK(((uintptr_t)offset & 3) == 0, "%s: offset must be 4-byte aligned", who);
   a.x = x; a.offset = offset; a.NB = NB; a.H = H; a.W = W; a.C = C; a.KH = KH; a.KW = KW; a.stride = stride;
   a.dil = dil; a.pad = pad; a.dgroups = dgroups; a.off_ld = off_ld;
-  a.Ho = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
-  a.Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+  a.Ho = (int)Ho;
+  a.Wo = (int)Wo;
   a.col = nullptr; a.dx = nullptr; a.doffset = nullptr; a.acc = nullptr;
+  return 0;
+}
+
+// the backward's outputs: dx is 4-byte aligned for the fp64-scratch entry (scalar adds) and 16-byte aligned for the
+// float4 atomics of the float-atomic entry; doffset takes single-float stores / atomics
+int check_bwd_out(const char* who, const float* dx, const float* doffset, uintptr_t dx_align) {
+  SN_CHECK(dx != nullptr && doffset != nullptr, "%s: dx / doffset must not be null", who);
+  SN_CHECK(((uintptr_t)dx & (dx_align - 1)) == 0, "%s: dx must be %d-byte aligned", who, (int)dx_align);
+  SN_CHECK(((uintptr_t)doffset & 3) == 0, "%s: doffset must be 4-byte aligned", who);
   return 0;
 }
 
@@ -200,8 +233,8 @@ extern "C" {
 int sniper_deform_im2col(const void* x, const float* offset, int NB, int H, int W, int C, int KH, int KW, int stride,
                          int dil, int pad, int dgroups, int off_ld, void* col, int dtype, void* stream) {
   DcArgs a;
-  SN_CHECK(dtype == 0 || dtype == 1, "deform_im2col: dtype must be 0 (fp32) or 1 (bf16)");
-  if (fill(a, x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld)) return -1;
+  if (fill(a, "deform_im2col", x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld, col, dtype)) return -1;
+  if (NB == 0) return 0;
   a.col = col;
   if (dtype == 0) deform_im2col_kernel<false, float><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);
   else deform_im2col_kernel<false, bf16><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);
@@ -216,8 +249,10 @@ int sniper_deform_col2im(const void* dcol, const void* x, const float* offset, i
                          int KW, int stride, int dil, int pad, int dgroups, int off_ld, float* dx, float* doffset,
                          int dtype, void* stream) {
   DcArgs a;
-  SN_CHECK(dtype == 0 || dtype == 1, "deform_col2im: dtype must be 0 (fp32) or 1 (bf16)");
-  if (fill(a, x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld)) return -1;
+  if (fill(a, "deform_col2im", x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld, dcol, dtype))
+    return -1;
+  if (check_bwd_out("deform_col2im", dx, doffset, 16)) return -1;
+  if (NB == 0) return 0;
   a.col = const_cast<void*>(dcol); a.dx = dx; a.doffset = doffset;
   if (dtype == 0) deform_im2col_kernel<true, float><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);
   else deform_im2col_kernel<true, bf16><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);
@@ -234,10 +269,13 @@ int sniper_deform_col2im_fp64acc(const void* dcol, const void* x, const float* o
                                  int KH, int KW, int stride, int dil, int pad, int dgroups, int off_ld, float* dx,
                                  float* doffset, int dtype, double* acc, long acc_elems, void* stream) {
   DcArgs a;
-  SN_CHECK(dtype == 0 || dtype == 1, "deform_col2im: dtype must be 0 (fp32) or 1 (bf16)");
+  if (fill(a, "deform_col2im_fp64acc", x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld, dcol, dtype))
+    return -1;
+  if (check_bwd_out("deform_col2im_fp64acc", dx, doffset, 4)) return -1;
   const long n = (long)NB * H * W * C;
   SN_CHECK(acc != nullptr && acc_elems >= n, "deform_col2im_fp64acc: acc needs %ld elements, %ld given", n, acc_elems);
-  if (fill(a, x, offset, NB, H, W, C, KH, KW, stride, dil, pad, dgroups, off_ld)) return -1;
+  SN_CHECK(((uintptr_t)acc & 7) == 0, "deform_col2im_fp64acc: acc must be 8-byte aligned");
+  if (NB == 0) return 0;
   a.col = const_cast<void*>(dcol); a.dx = dx; a.doffset = doffset; a.acc = acc;
   if (dtype == 0) deform_im2col_kernel<true, float><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);
   else deform_im2col_kernel<true, bf16><<<dc_grid(a), 256, 0, (cudaStream_t)stream>>>(a);

@@ -465,11 +465,13 @@ __global__ void __launch_bounds__(256) deform_psroi_fwd_sep_nhwc_kernel(PsArgs p
   }
 }
 
+// The warp-per-bin kernels read data and write top_data / top_count as float4: every such buffer must be 16-byte
+// aligned, otherwise the call takes the generic per-output kernel.
 bool fast_nhwc_ok(const PsArgs& a) {
   return a.layout == 1 && a.group_size == 1 && a.num_classes == 1 && a.sample_idx == nullptr &&
          a.sample_per_part <= 4 &&
          (a.channels == 128 || a.channels == 256 || a.channels == 512) &&
-         ((uintptr_t)a.data & 15) == 0;
+         ((uintptr_t)a.data & 15) == 0 && ((uintptr_t)a.top_data & 15) == 0 && ((uintptr_t)a.top_count & 15) == 0;
 }
 
 int fast_grid(long nbins) {
@@ -552,6 +554,14 @@ int fill_common(PsArgs& a, const float* data, const float* rois, const float* tr
                 int height, int width, float spatial_scale, int output_dim, int group_size, int pooled_size,
                 int part_size, int sample_per_part, float trans_std, int no_trans, int num_classes, int layout) {
   SN_CHECK(layout == 0 || layout == 1, "psroi: layout must be 0 (NCHW) or 1 (NHWC)");
+  SN_CHECK(num_rois >= 0, "psroi: num_rois (%d) must not be negative", num_rois);
+  SN_CHECK(height >= 1 && width >= 1, "psroi: height (%d) and width (%d) must be at least 1", height, width);
+  SN_CHECK(output_dim >= 1, "psroi: output_dim (%d) must be at least 1", output_dim);
+  SN_CHECK(group_size >= 1, "psroi: group_size (%d) must be at least 1", group_size);
+  SN_CHECK(pooled_size >= 1, "psroi: pooled_size (%d) must be at least 1", pooled_size);
+  SN_CHECK(part_size >= 0, "psroi: part_size (%d) must not be negative", part_size);
+  SN_CHECK(sample_per_part >= 1, "psroi: sample_per_part (%d) must be at least 1", sample_per_part);
+  SN_CHECK(rois != nullptr, "psroi: rois must not be null");
   SN_CHECK(channels == output_dim * group_size * group_size, "psroi: channels (%d) != output_dim*group_size^2 (%d)",
            channels, output_dim * group_size * group_size);
   SN_CHECK(no_trans || (trans != nullptr && num_classes > 0 && output_dim % num_classes == 0),
@@ -580,6 +590,7 @@ int sniper_deform_psroi_fwd(const float* data, const float* rois, const float* t
   if (fill_common(a, data, rois, trans, num_rois, channels, height, width, spatial_scale, output_dim, group_size,
                   pooled_size, part_size, sample_per_part, trans_std, no_trans, num_classes, layout))
     return -1;
+  SN_CHECK(data != nullptr && top_data != nullptr, "deform_psroi_fwd: data / top_data must not be null");
   a.top_data = top_data; a.top_count = top_count; a.sample_idx = sample_idx;
   const long count = (long)num_rois * output_dim * pooled_size * pooled_size;
   if (count == 0) return 0;
@@ -615,6 +626,8 @@ int sniper_deform_psroi_bwd(const float* top_diff, const float* data, const floa
                   pooled_size, part_size, sample_per_part, trans_std, no_trans, num_classes, layout))
     return -1;
   SN_CHECK(no_trans || trans_diff != nullptr, "deformable psroi bwd: trans_diff is null");
+  SN_CHECK(top_diff != nullptr && data != nullptr && data_diff != nullptr,
+           "deform_psroi_bwd: top_diff / data / data_diff must not be null");
   a.top_diff = top_diff; a.data_diff = data_diff; a.trans_diff = trans_diff;
   a.acc = nullptr; a.data_elems = 0;
   const long count = (long)num_rois * output_dim * pooled_size * pooled_size;
@@ -651,6 +664,9 @@ int sniper_deform_psroi_bwd_fp64acc(const float* top_diff, const float* data, co
                   pooled_size, part_size, sample_per_part, trans_std, no_trans, num_classes, 1))
     return -1;
   SN_CHECK(no_trans || trans_diff != nullptr, "deformable psroi bwd: trans_diff is null");
+  SN_CHECK(top_diff != nullptr && data != nullptr && data_diff != nullptr,
+           "deform_psroi_bwd_fp64acc: top_diff / data / data_diff must not be null");
+  SN_CHECK(batch >= 1, "deform_psroi_bwd_fp64acc: batch (%d) must be at least 1", batch);
   a.top_diff = top_diff; a.data_diff = data_diff; a.trans_diff = trans_diff;
   if (!fast_nhwc_ok(a) || ((uintptr_t)data_diff & 15) != 0 || ((uintptr_t)top_diff & 15) != 0) {
     sn::set_error("deformable psroi bwd fp64acc: shape / alignment does not qualify for the NHWC kernels");
@@ -660,6 +676,7 @@ int sniper_deform_psroi_bwd_fp64acc(const float* top_diff, const float* data, co
   const long trans_elems = no_trans ? 0 : (long)num_rois * 2 * a.part_size * a.part_size;
   SN_CHECK(acc != nullptr && acc_elems >= data_elems + trans_elems,
            "deformable psroi bwd fp64acc: acc needs %ld elements, %ld given", data_elems + trans_elems, acc_elems);
+  SN_CHECK(((uintptr_t)acc & 7) == 0, "deform_psroi_bwd_fp64acc: acc must be 8-byte aligned");
   a.acc = acc; a.data_elems = data_elems;
   const long nbins = (long)num_rois * pooled_size * pooled_size;
   if (nbins == 0) return 0;
@@ -685,6 +702,7 @@ int sniper_psroi_fwd(const float* data, const float* rois, int num_rois, int cha
   if (fill_common(a, data, rois, nullptr, num_rois, channels, height, width, spatial_scale, output_dim, group_size,
                   pooled_size, pooled_size, 1, 0.0f, 1, 1, layout))
     return -1;
+  SN_CHECK(data != nullptr && top_data != nullptr, "psroi_fwd: data / top_data must not be null");
   a.top_data = top_data; a.sample_idx = bins;
   const long count = (long)num_rois * output_dim * pooled_size * pooled_size;
   if (count == 0) return 0;
@@ -700,6 +718,7 @@ int sniper_psroi_bwd(const float* top_diff, const float* rois, int num_rois, int
   if (fill_common(a, nullptr, rois, nullptr, num_rois, channels, height, width, spatial_scale, output_dim, group_size,
                   pooled_size, pooled_size, 1, 0.0f, 1, 1, layout))
     return -1;
+  SN_CHECK(top_diff != nullptr && data_diff != nullptr, "psroi_bwd: top_diff / data_diff must not be null");
   a.top_diff = top_diff; a.data_diff = data_diff;
   const long count = (long)num_rois * output_dim * pooled_size * pooled_size;
   if (count == 0) return 0;
