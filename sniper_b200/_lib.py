@@ -42,6 +42,8 @@ SIGNATURES = {
     "sniper_affine_relu_bwd": ("i", "plplpp" "pl" "pl" "lii" "p"),
     "sniper_depthwise3x3_fwd": ("i", "plppl" "iiiiii" "p"),
     "sniper_depthwise3x3_dgrad": ("i", "plppl" "iiiiii" "p"),
+    "sniper_depthwise3x3_wgrad_workspace_bytes": ("z", ""),
+    "sniper_depthwise3x3_set_wgrad_workspace": ("i", "pzip"),
     "sniper_depthwise3x3_wgrad": ("i", "plplp" "iiiiii" "p"),
     "sniper_im2col3x3s2_nchw": ("i", "pp" "iiiiii" "p"),
     "sniper_add_rows": ("i", "plplpl" "lii" "p"),
@@ -93,6 +95,8 @@ KERNELS_PER_CALL = {
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
     "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
+    "sniper_depthwise3x3_wgrad_workspace_bytes": 0, "sniper_depthwise3x3_set_wgrad_workspace": 0,
+    "sniper_depthwise3x3_wgrad": 2,
 }
 launches = [0]
 

@@ -60,12 +60,15 @@ __global__ void __launch_bounds__(kTPB) dw_dgrad_s2_kernel(const T* __restrict__
 }
 
 // block = 32 x 8 threads; a warp row covers LC channel vectors x 32/LC strips (depthwise_core.cuh).  Partial sums of
-// the strip lanes are combined in shared memory, then one float atomic per (block, tap, channel): gridDim.x * 9 * C
-// atomics in total.  The grid is ONE wave of resident blocks (occupancy API): each thread loops over its strips.
+// the strip lanes are combined in shared memory, then each block stores its [9 x its channels] partial to row blockIdx.x
+// of a slab part[gridDim.x][9][C] in the caller's workspace; dw_wgrad_reduce_kernel adds the rows in a fixed order.  No
+// atomics: the result does not depend on the order in which blocks run, so two launches give the same bits.  The grid
+// is ONE wave of resident blocks (occupancy API), capped so that the slab fits the workspace; each thread loops over
+// its strips.
 constexpr int kWgTY = 8;
 template <typename T, int S, int PW>
 __global__ void __launch_bounds__(32 * kWgTY) dw_wgrad_kernel(const T* __restrict__ x, const T* __restrict__ dy,
-                                                               float* __restrict__ dw, dwc::Params p) {
+                                                               float* __restrict__ part, dwc::Params p) {
   __shared__ float red[kWgTY][32][37];
   const int tx = threadIdx.x, ty = threadIdx.y;
   float acc[9][4];
@@ -76,6 +79,7 @@ __global__ void __launch_bounds__(32 * kWgTY) dw_wgrad_kernel(const T* __restric
     for (int k = 0; k < 4; ++k) red[ty][tx][t * 4 + k] = acc[t][k];
   __syncthreads();
   const int LC = dwc::wgrad_lc(p.C), PPW = 32 / LC;
+  float* row = part + (long)blockIdx.x * 9 * p.C;
   for (int i = ty * 32 + tx; i < LC * 36; i += 32 * kWgTY) {
     const int lane = i / 36, e = i - lane * 36;
     float s = 0.f;
@@ -83,9 +87,51 @@ __global__ void __launch_bounds__(32 * kWgTY) dw_wgrad_kernel(const T* __restric
 #pragma unroll
       for (int j = 0; j < kWgTY; ++j) s += red[j][ps * LC + lane][e];
     const int c = (((int)blockIdx.y * LC + lane) << 2) + (e & 3);
-    if (c < p.C && s != 0.f) atomicAdd(dw + (long)(e >> 2) * p.C + c, s);
+    if (c < p.C) row[(e >> 2) * p.C + c] = s;
   }
 }
+
+// dw[o] += sum over b of part[b][o], o < n = 9 C, in a fixed order: thread row ty sums the contiguous block range
+// [gx*ty/8, gx*(ty+1)/8) in increasing b, then row 0 adds the 8 row sums in increasing ty and adds the total to dw
+// once.  Block = 32 outputs x 8 rows; the 32 lanes of a warp read 32 consecutive floats of a slab row.
+constexpr int kRdTY = 8;
+__global__ void __launch_bounds__(32 * kRdTY) dw_wgrad_reduce_kernel(const float* __restrict__ part, int gx, int n,
+                                                                      float* __restrict__ dw) {
+  __shared__ float red[kRdTY][32];
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int o = (int)blockIdx.x * 32 + tx;
+  float s = 0.f;
+  if (o < n) {
+    const int b0 = gx * ty / kRdTY, b1 = gx * (ty + 1) / kRdTY;
+#pragma unroll 8
+    for (int b = b0; b < b1; ++b) s += part[(long)b * n + o];
+  }
+  red[ty][tx] = s;
+  __syncthreads();
+  if (ty == 0 && o < n) {
+    float t = red[0][tx];
+#pragma unroll
+    for (int j = 1; j < kRdTY; ++j) t += red[j][tx];
+    dw[o] += t;
+  }
+}
+
+// Workspace of one launch: the slab holds at most kWgSlabFloats partials.  The one-wave grid needs about
+// kNumSMs * (blocks per SM) * 9 * 128 floats (a block covers at most 128 channels); at 126..158 registers per thread
+// that is 1..2 blocks per SM, so the cap (4 blocks per SM) binds only for grids the occupancy rule would not pick.
+constexpr long kWgSlabFloats = (long)sn::kNumSMs * 4 * 9 * 128;
+
+// Caller-owned workspaces, one per (device, stream): launches on one stream run one after another and can share a
+// slab; launches on different streams may overlap and must not.  Host-side table; like the GEMM's split-K table the
+// entry points are not re-entrant across host threads (one host thread drives a device's launches).
+constexpr int kWgWsEntries = 256;
+struct WgWs {
+  int device;
+  cudaStream_t stream;
+  void* ws;
+};
+WgWs g_wg_ws[kWgWsEntries];
+int g_wg_ws_n = 0;
 
 template <typename K>
 int wgrad_blocks_per_sm(K kernel) {
@@ -182,28 +228,83 @@ int sniper_depthwise3x3_dgrad(const void* dy, long lddy, const float* w, void* d
   return 0;
 }
 
-// dw[9,C] += sum over pixels of dy * shifted x  (fp32, accumulated with atomics: zero it for kWriteTo).
+// Bytes of the workspace sniper_depthwise3x3_set_wgrad_workspace expects (the same for every shape).
+size_t sniper_depthwise3x3_wgrad_workspace_bytes(void) { return (size_t)kWgSlabFloats * sizeof(float); }
+
+// Registers a caller-owned device buffer of sniper_depthwise3x3_wgrad_workspace_bytes() bytes (16-byte aligned, no
+// initialisation needed) for the weight-gradient launches enqueued on `stream` of `device`; it must outlive them.
+// Registering again for the same (device, stream) replaces the buffer.  The library itself never allocates.
+int sniper_depthwise3x3_set_wgrad_workspace(void* ws, size_t bytes, int device, void* stream) {
+  SN_CHECK(device >= 0, "depthwise3x3_set_wgrad_workspace: device (%d) must be >= 0", device);
+  SN_CHECK(ws != nullptr, "depthwise3x3_set_wgrad_workspace: ws must not be null");
+  SN_CHECK((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "depthwise3x3_set_wgrad_workspace: ws must be 16-byte aligned");
+  SN_CHECK(bytes >= sniper_depthwise3x3_wgrad_workspace_bytes(),
+           "depthwise3x3_set_wgrad_workspace: bytes (%zu) is smaller than sniper_depthwise3x3_wgrad_workspace_bytes() (%zu)",
+           bytes, sniper_depthwise3x3_wgrad_workspace_bytes());
+  const cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < g_wg_ws_n; ++i)
+    if (g_wg_ws[i].device == device && g_wg_ws[i].stream == st) {
+      g_wg_ws[i].ws = ws;
+      return 0;
+    }
+  SN_CHECK(g_wg_ws_n < kWgWsEntries, "depthwise3x3_set_wgrad_workspace: more than %d (device, stream) pairs",
+           kWgWsEntries);
+  g_wg_ws[g_wg_ws_n++] = WgWs{device, st, ws};
+  return 0;
+}
+
+// dw[9,C] += sum over pixels of dy * shifted x (fp32; one addition into the existing value: zero dw for kWriteTo).
+// The block partials go through the workspace registered for (current device, stream) and are added in a fixed
+// order, so every launch gives the same bits.
 int sniper_depthwise3x3_wgrad(const void* x, long ldx, const void* dy, long lddy, float* dw, int NB, int H, int W,
                               int C, int stride, int dtype, void* stream) {
+  SN_CHECK(dtype == 0 || dtype == 1, "depthwise3x3_wgrad: dtype (%d) must be 0 (fp32) or 1 (bf16)", dtype);
+  SN_CHECK(stride == 1 || stride == 2, "depthwise3x3_wgrad: stride (%d) must be 1 or 2", stride);
+  SN_CHECK(NB > 0 && H > 0 && W > 0, "depthwise3x3_wgrad: NB (%d), H (%d) and W (%d) must be positive", NB, H, W);
+  SN_CHECK(C > 0 && C % 4 == 0, "depthwise3x3_wgrad: C (%d) must be a positive multiple of 4", C);
+  SN_CHECK(ldx >= C && ldx % 4 == 0, "depthwise3x3_wgrad: ldx (%ld) must be a multiple of 4 and >= C (%d)", ldx, C);
+  SN_CHECK(lddy >= C && lddy % 4 == 0, "depthwise3x3_wgrad: lddy (%ld) must be a multiple of 4 and >= C (%d)", lddy, C);
   dwc::Params p;
   if (fill_params(p, NB, H, W, C, stride, ldx, lddy, dtype, "depthwise3x3_wgrad")) return -1;
+  SN_CHECK(x != nullptr, "depthwise3x3_wgrad: x must not be null");
+  SN_CHECK(dy != nullptr, "depthwise3x3_wgrad: dy must not be null");
+  const uintptr_t vec = dtype == 0 ? 16 : 8;          // x and dy are read as 4-channel vectors
+  SN_CHECK(reinterpret_cast<uintptr_t>(x) % vec == 0, "depthwise3x3_wgrad: x must be %d-byte aligned", (int)vec);
+  SN_CHECK(reinterpret_cast<uintptr_t>(dy) % vec == 0, "depthwise3x3_wgrad: dy must be %d-byte aligned", (int)vec);
+  SN_CHECK(dw != nullptr, "depthwise3x3_wgrad: dw must not be null");
+  SN_CHECK((reinterpret_cast<uintptr_t>(dw) & 3) == 0, "depthwise3x3_wgrad: dw must be 4-byte aligned");
+  SN_CHECK(9L * C <= kWgSlabFloats, "depthwise3x3_wgrad: C (%d) exceeds the workspace's %ld channels", C,
+           kWgSlabFloats / 9);
   cudaStream_t st = (cudaStream_t)stream;
+  bool any = false;
+  for (int i = 0; i < g_wg_ws_n; ++i) any |= g_wg_ws[i].stream == st;
+  SN_CHECK(any, "depthwise3x3_wgrad: no workspace registered for this stream (sniper_depthwise3x3_set_wgrad_workspace)");
+  int dev = -1;
+  SN_CUDA(cudaGetDevice(&dev));
+  float* part = nullptr;
+  for (int i = 0; i < g_wg_ws_n; ++i)
+    if (g_wg_ws[i].device == dev && g_wg_ws[i].stream == st) part = static_cast<float*>(g_wg_ws[i].ws);
+  SN_CHECK(part != nullptr, "depthwise3x3_wgrad: no workspace registered for device %d and this stream", dev);
   const int LC = dwc::wgrad_lc(C), PL = kWgTY * (32 / LC);
   const int gy = sn::div_up(C >> 2, LC);
   const dim3 block(32, kWgTY, 1);
+  long gx = 1;
 #define DW_WG(T, S, PW)                                                                                              \
   do {                                                                                                               \
     const long strips = (long)NB * p.Ho * ((p.Wo + PW - 1) / PW);                                                    \
-    long gx = ((long)sn::kNumSMs * wgrad_blocks_per_sm(dw_wgrad_kernel<T, S, PW>) + gy - 1) / gy;   /* one wave */    \
+    gx = ((long)sn::kNumSMs * wgrad_blocks_per_sm(dw_wgrad_kernel<T, S, PW>) + gy - 1) / gy;   /* one wave */         \
     const long gx_max = (strips + PL - 1) / PL;                                                                      \
     if (gx > gx_max) gx = gx_max;                                                                                    \
+    if (gx > kWgSlabFloats / (9L * C)) gx = kWgSlabFloats / (9L * C);                                                \
     if (gx < 1) gx = 1;                                                                                              \
     dw_wgrad_kernel<T, S, PW><<<dim3((unsigned)gx, (unsigned)gy, 1), block, 0, st>>>(                                \
-        static_cast<const T*>(x), static_cast<const T*>(dy), dw, p);                                                \
+        static_cast<const T*>(x), static_cast<const T*>(dy), part, p);                                              \
   } while (0)
   if (dtype == 0) { if (stride == 1) DW_WG(float, 1, 4); else DW_WG(float, 2, 2); }
   else            { if (stride == 1) DW_WG(bf16, 1, 4);  else DW_WG(bf16, 2, 2); }
 #undef DW_WG
+  const int n = 9 * C;
+  dw_wgrad_reduce_kernel<<<(unsigned)sn::div_up(n, 32), dim3(32, kRdTY, 1), 0, st>>>(part, (int)gx, n, dw);
   SN_LAUNCH_CHECK();
   return 0;
 }

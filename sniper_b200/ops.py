@@ -945,11 +945,30 @@ def depthwise3x3_dgrad(dy, w, in_hw, stride=1, out=None):
     return out
 
 
+_dw_ws = {}
+
+
+def _ensure_dw_wgrad_workspace():
+    """The depthwise weight gradient sums its block partials in a caller-owned slab (the library never allocates): one
+    buffer per (device, stream), because launches on different streams (WgradScheduler's side stream, the main
+    stream) may overlap.  Registered once and kept alive for the life of the process, so that captured CUDA graphs
+    keep a valid address."""
+    idx, st = torch.cuda.current_device(), _stream()
+    if (idx, st) not in _dw_ws:
+        L = lib()
+        n = L.sniper_depthwise3x3_wgrad_workspace_bytes()
+        buf = torch.empty(n, dtype=torch.uint8, device=torch.device("cuda", idx))
+        check(L.sniper_depthwise3x3_set_wgrad_workspace(buf.data_ptr(), n, idx, st))
+        _dw_ws[(idx, st)] = buf
+
+
 def depthwise3x3_wgrad(x, dy, dw, stride=1):
-    """dw[9,C] (fp32) += correlation of dy with the shifted input."""
+    """dw[9,C] (fp32) += correlation of dy with the shifted input, summed in a fixed order (two calls give the same
+    bits)."""
     NB, H, W, C = x.shape
     assert dw.shape == (9, C) and dw.dtype == torch.float32 and dw.is_contiguous() and x.dtype == dy.dtype
     assert x.is_contiguous() and dy.is_contiguous()
+    _ensure_dw_wgrad_workspace()
     check(lib().sniper_depthwise3x3_wgrad(_ptr(x), x.stride(2), _ptr(dy), dy.stride(2), _ptr(dw), NB, H, W, C, stride,
                                           _sdt(x), _stream()))
     return dw

@@ -34,7 +34,9 @@ DOC = {
     "sniper_affine_relu_bwd": "Backward of relu?(x*scale+shift) for frozen BN.",
     "sniper_depthwise3x3_fwd": "Depthwise 3x3 convolution, pad 1, stride 1|2, NHWC, weights [9,C] fp32: Convolution(num_group = num_filter = C) of mobilenetv2_e2e.py:58-66 (src/operator/nn/depthwise_convolution-inl.h DepthwiseConvolutionOp::Forward).",
     "sniper_depthwise3x3_dgrad": "Data gradient of the depthwise convolution (depthwise_convolution-inl.h Backward, DepthwiseConv2dBackwardDataGpu), gather form.",
-    "sniper_depthwise3x3_wgrad": "Weight gradient of the depthwise convolution (DepthwiseConv2dBackwardFilterGpu): dw[9,C] += per-channel correlation of dy with the shifted input.",
+    "sniper_depthwise3x3_wgrad_workspace_bytes": "Size of the caller-owned scratch one sniper_depthwise3x3_wgrad launch uses (the same for every shape).",
+    "sniper_depthwise3x3_set_wgrad_workspace": "Registers that scratch (caller-owned, no initialisation, must outlive later launches) for the weight-gradient launches on one (device, stream); the library itself never allocates device memory.",
+    "sniper_depthwise3x3_wgrad": "Weight gradient of the depthwise convolution (DepthwiseConv2dBackwardFilterGpu): dw[9,C] += per-channel correlation of dy with the shifted input; block partials summed in a fixed order through the registered scratch (bit-reproducible).",
     "sniper_im2col3x3s2_nchw": "im2col of MobileNetV2's first layer (3x3 / stride 2 / pad 1 over the 3-channel fp32 NCHW `data`, mobilenetv2_e2e.py:204-212) so that it runs on the wgmma GEMM; K order (kh, kw, ci), zero-padded to Kp.",
     "sniper_add_rows": "out = a + b on [M,C] rows: elemwise_add of the inverted-residual shortcut (mobilenetv2_e2e.py:22-24).",
     "sniper_relu_bwd": "dx = dy * (y > 0).",
