@@ -402,70 +402,99 @@ __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoor
     col_base = tap * (p.wg_cin_blocks * p.block_n) + (tc.tile_n - tap * p.wg_cin_blocks) * p.block_n;
   }
   const __nv_bfloat16* res16 = reinterpret_cast<const __nv_bfloat16*>(p.residual);
+  // The residual may be the output itself (an in-place sum), so the compiler may not move a residual load above an
+  // earlier store: loaded one pair at a time, each load would wait out a full memory round trip.  The residual of
+  // kResChunk column blocks is therefore loaded into registers before any of their stores (each thread reads only the
+  // elements it writes itself), which keeps 4 * kResChunk loads in flight per thread.
+  constexpr int kResChunk = 8;
+  static_assert((W / 8) % kResChunk == 0, "residual chunks");
 #pragma unroll
-  for (int j = 0; j < W / 8; ++j) {
-    const int n = col_base + 8 * j + cq;
-    float sm0 = 0.f, sm1 = 0.f, sq0 = 0.f, sq1 = 0.f;
-    if (n < p.N) {
-      const bool two = n + 1 < p.N;
-      const float sc0 = p.scale ? __ldg(p.scale + n) : 1.f, sc1 = (p.scale && two) ? __ldg(p.scale + n + 1) : 1.f;
-      const float bi0 = p.bias ? __ldg(p.bias + n) : 0.f, bi1 = (p.bias && two) ? __ldg(p.bias + n + 1) : 0.f;
+  for (int j0 = 0; j0 < W / 8; j0 += kResChunk) {
+    float res[kResChunk][4];
+    if (p.residual) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h]) continue;
-        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-        if (p.scale) { x0 *= sc0; x1 *= sc1; }
-        if (p.bias) { x0 += bi0; x1 += bi1; }
-        const long ro = row[h];
-        if (p.residual) {
-          // bf16 output implies a bf16 residual (mixed-precision activations); fp32 otherwise
-          if (p.out_bf16) {
-            x0 += __bfloat162float(res16[ro * p.ldr + n]);
-            if (two) x1 += __bfloat162float(res16[ro * p.ldr + n + 1]);
-          } else {
-            x0 += p.residual[ro * p.ldr + n];
-            if (two) x1 += p.residual[ro * p.ldr + n + 1];
+      for (int jj = 0; jj < kResChunk; ++jj) {
+        const int n = col_base + 8 * (j0 + jj) + cq;
+        const bool two = n + 1 < p.N;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float r0 = 0.f, r1 = 0.f;
+          if (n < p.N && row_ok[h]) {
+            // bf16 output implies a bf16 residual (mixed-precision activations); fp32 otherwise
+            const long ri = row[h] * p.ldr + n;
+            if (p.out_bf16) {
+              r0 = __bfloat162float(res16[ri]);
+              if (two) r1 = __bfloat162float(res16[ri + 1]);
+            } else {
+              r0 = p.residual[ri];
+              if (two) r1 = p.residual[ri + 1];
+            }
           }
-        }
-        if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-        if (p.out_bf16) {
-          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.C) + ro * p.ldc + n;
-          const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
-          x0 = __low2float(h2);   // statistics of the values the consumer reads
-          x1 = __high2float(h2);
-          if (two && (reinterpret_cast<uintptr_t>(o) & 3) == 0) *reinterpret_cast<__nv_bfloat162*>(o) = h2;
-          else { o[0] = __low2bfloat16(h2); if (two) o[1] = __high2bfloat16(h2); }
-        } else {
-          float* o = p.C + ro * p.ldc + n;
-          if (p.atomic) {
-            atomicAdd(o, x0);
-            if (two) atomicAdd(o + 1, x1);
-          } else if (two && (reinterpret_cast<uintptr_t>(o) & 7) == 0) {
-            *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
-          } else {
-            o[0] = x0;
-            if (two) o[1] = x1;
-          }
-        }
-        if (f_stats) {
-          sm0 += x0; sq0 = fmaf(x0, x0, sq0);
-          if (two) { sm1 += x1; sq1 = fmaf(x1, x1, sq1); }
+          res[jj][2 * h] = r0;
+          res[jj][2 * h + 1] = r1;
         }
       }
     }
-    if (f_stats) {
-      // column sums over the warp's 16 rows (lanes with equal lane & 3 hold the same columns), then over the CTA
 #pragma unroll
-      for (int o = 4; o < 32; o <<= 1) {
-        sm0 += __shfl_xor_sync(0xffffffffu, sm0, o);
-        sm1 += __shfl_xor_sync(0xffffffffu, sm1, o);
-        sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
-        sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
+    for (int jj = 0; jj < kResChunk; ++jj) {
+      const int j = j0 + jj;
+      const int n = col_base + 8 * j + cq;
+      float sm0 = 0.f, sm1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+      if (n < p.N) {
+        const bool two = n + 1 < p.N;
+        const float sc0 = p.scale ? __ldg(p.scale + n) : 1.f, sc1 = (p.scale && two) ? __ldg(p.scale + n + 1) : 1.f;
+        const float bi0 = p.bias ? __ldg(p.bias + n) : 0.f, bi1 = (p.bias && two) ? __ldg(p.bias + n + 1) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h]) continue;
+          float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+          if (p.scale) { x0 *= sc0; x1 *= sc1; }
+          if (p.bias) { x0 += bi0; x1 += bi1; }
+          const long ro = row[h];
+          if (p.residual) {
+            x0 += res[jj][2 * h];
+            if (two) x1 += res[jj][2 * h + 1];
+          }
+          if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+          if (p.out_bf16) {
+            __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.C) + ro * p.ldc + n;
+            const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
+            x0 = __low2float(h2);   // statistics of the values the consumer reads
+            x1 = __high2float(h2);
+            if (two && (reinterpret_cast<uintptr_t>(o) & 3) == 0) *reinterpret_cast<__nv_bfloat162*>(o) = h2;
+            else { o[0] = __low2bfloat16(h2); if (two) o[1] = __high2bfloat16(h2); }
+          } else {
+            float* o = p.C + ro * p.ldc + n;
+            if (p.atomic) {
+              atomicAdd(o, x0);
+              if (two) atomicAdd(o + 1, x1);
+            } else if (two && (reinterpret_cast<uintptr_t>(o) & 7) == 0) {
+              *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
+            } else {
+              o[0] = x0;
+              if (two) o[1] = x1;
+            }
+          }
+          if (f_stats) {
+            sm0 += x0; sq0 = fmaf(x0, x0, sq0);
+            if (two) { sm1 += x1; sq1 = fmaf(x1, x1, sq1); }
+          }
+        }
       }
-      if (lane < 4) {
-        // this warp's partial sums; summed over the 8 warps in a fixed order below (deterministic forward pass)
-        float* w = st_buf + (ct >> 5) * 512 + 8 * j + cq;
-        w[0] = sm0; w[1] = sm1; w[256] = sq0; w[257] = sq1;
+      if (f_stats) {
+        // column sums over the warp's 16 rows (lanes with equal lane & 3 hold the same columns), then over the CTA
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          sm0 += __shfl_xor_sync(0xffffffffu, sm0, o);
+          sm1 += __shfl_xor_sync(0xffffffffu, sm1, o);
+          sq0 += __shfl_xor_sync(0xffffffffu, sq0, o);
+          sq1 += __shfl_xor_sync(0xffffffffu, sq1, o);
+        }
+        if (lane < 4) {
+          // this warp's partial sums; summed over the 8 warps in a fixed order below (deterministic forward pass)
+          float* w = st_buf + (ct >> 5) * 512 + 8 * j + cq;
+          w[0] = sm0; w[1] = sm1; w[256] = sq0; w[257] = sq1;
+        }
       }
     }
   }
