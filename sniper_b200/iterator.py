@@ -462,16 +462,28 @@ def synthetic_roidb(n_images, seed=0, width=1333, height=800, n_gt=(1, 20), n_pr
 def default_config(neg=True, autofocus=False, network="resnet101"):
     """The slice of configs/faster/sniper_res101_e2e.yml the iterator reads (:21-39, 76-101, 120-140); autofocus=True:
     TRAIN.AUTO_FOCUS of configs/faster/sniper_res101_e2e_autofocus.yml (FocusPixel labels, thresholds 5 / 64 / 90).
-    network="mobilenetv2": the network block of configs/faster/sniper_mobilenetv2_e2e.yml instead (stride 32, scales
-    1 / 2 / 4 / 8 / 12: 15 anchors), for model_mnv2.SniperMobileNetV2."""
+    network="mobilenetv2": the network and TEST blocks of configs/faster/sniper_mobilenetv2_e2e.yml instead (stride 32,
+    scales 1 / 2 / 4 / 8 / 12: 15 anchors; plain multi-scale inference without AutoFocus), for
+    model_mnv2.SniperMobileNetV2."""
     import types
     S = types.SimpleNamespace
     if network == "resnet101":
         net = S(PIXEL_MEANS=[103.06, 115.90, 123.15], ANCHOR_SCALES=[2, 4, 7, 10, 13, 16, 24], ANCHOR_RATIOS=[0.5, 1, 2],
                 RPN_FEAT_STRIDE=16, NUM_ANCHORS=21)
+        # TEST block of configs/faster/sniper_res101_e2e_autofocus.yml:191-245 (AutoFocus inference, BASELINE config 5)
+        test = S(SCALES=[(480, 512), (800, 1280), (1400, 2000)], BATCH_IMAGES=[8, 8, 2], MAX_PER_IMAGE=200,
+                 VALID_RANGES=[(75, -1), (32, 180), (-1, 75)], AUTO_FOCUS=True, DO_PRUNING=[False, True, True],
+                 CHIP_HYPERPARAMS=[(3, 0.02, 16), (3, 0.2, 20)], NMS=0.45, NMS_SIGMA=0.55)
     elif network == "mobilenetv2":
         net = S(PIXEL_MEANS=[103.939, 116.779, 123.68], ANCHOR_SCALES=[1, 2, 4, 8, 12], ANCHOR_RATIOS=[0.5, 1, 2],
                 RPN_FEAT_STRIDE=32, NUM_ANCHORS=15)
+        # TEST block of configs/faster/sniper_mobilenetv2_e2e.yml:179-256; AUTO_FOCUS / DO_PRUNING / CHIP_HYPERPARAMS are
+        # not in the yml and keep configs/faster/default_configs.py's values.  NMS -1 reaches only the soft-NMS's
+        # linear / hard branches; the aggregation runs the Gaussian one (method 2), which reads NMS_SIGMA.
+        test = S(SCALES=[(1400, 2000), (800, 1280), (480, 512)], BATCH_IMAGES=[2, 2, 4], MAX_PER_IMAGE=200,
+                 VALID_RANGES=[(-1, 90), (32, 180), (75, -1)], AUTO_FOCUS=False, DO_PRUNING=[False, False, False],
+                 CHIP_HYPERPARAMS=[(-1, -1, -1), (-1, -1, -1), (-1, -1, -1)], NMS=-1, NMS_SIGMA=0.55,
+                 RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, RPN_MIN_SIZE=0)
     else:
         raise ValueError("default_config: network must be 'resnet101' or 'mobilenetv2', not %r" % (network,))
     return S(network=net,
@@ -479,8 +491,5 @@ def default_config(neg=True, autofocus=False, network="resnet101"):
                      CPP_CHIPS=True, USE_NEG_CHIPS=neg, RPN_BATCH_SIZE=256, RPN_FG_FRACTION=0.5,
                      RPN_POSITIVE_OVERLAP=0.5, RPN_NEGATIVE_OVERLAP=0.4, BATCH_IMAGES=16, AUTO_FOCUS=autofocus,
                      AUTO_FOCUS_DC_LOW=5, AUTO_FOCUS_SMALL_THRESH=64, AUTO_FOCUS_DC_HIGH=90),
-             # TEST block of configs/faster/sniper_res101_e2e_autofocus.yml:191-245 (AutoFocus inference, BASELINE config 5)
-             TEST=S(SCALES=[(480, 512), (800, 1280), (1400, 2000)], BATCH_IMAGES=[8, 8, 2], MAX_PER_IMAGE=200,
-                    VALID_RANGES=[(75, -1), (32, 180), (-1, 75)], AUTO_FOCUS=True, DO_PRUNING=[False, True, True],
-                    CHIP_HYPERPARAMS=[(3, 0.02, 16), (3, 0.2, 20)], NMS=0.45, NMS_SIGMA=0.55),
+             TEST=test,
              dataset=S(NUM_CLASSES=81))

@@ -574,6 +574,10 @@ def head_bwd(net, x, rpn, dhead, dout, saved):
 class SniperResNet101:
     """get_symbol_rcnn(cfg, is_train=True) as an executable object (resnet_mx_101_e2e.py:227-345)."""
 
+    @property
+    def feat_stride(self):
+        return self.cfg.feat_stride
+
     def __init__(self, cfg=None, device="cuda", seed=5, deform_offset_std=0.0):
         self.cfg = cfg or Cfg()
         cfg = self.cfg

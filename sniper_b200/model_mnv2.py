@@ -167,6 +167,11 @@ class SniperMobileNetV2:
     # the R-CNN loss is not normalised by the valid count (:281-282), so cnt_buf[1] stays 0: the trainer's metric
     # launch counts the rows itself
     rcnn_valid_counted = False
+    af = None                         # the reference's MobileNetV2 graph has no FocusPixel branch (tester.DetectionNetwork)
+
+    @property
+    def feat_stride(self):
+        return self.cfg.feat_stride
 
     def __init__(self, cfg=None, device="cuda", seed=5):
         self.cfg = cfg or MCfg()
@@ -330,11 +335,14 @@ class SniperMobileNetV2:
                    bbox_target=bbox_target, bbox_weight=bbox_weight)
 
     # ---------------------------------------------------------------- inference graph
-    def forward_inference(self, data, im_info, rpn_pre_nms_top_n=6000):
+    def forward_inference(self, data, im_info, rpn_pre_nms_top_n=6000, autofocus=False):
         """mobilenetv2_e2e.get_symbol_rcnn(cfg, is_train=False) (:306-362): every BatchNorm on its moving statistics,
         SoftmaxActivation over the RPN scores, MultiProposal (TEST.RPN_PRE_NMS_TOP_N 6000, 300 rois per image, stride 32),
         deformable R-FCN head -> (rois [B*R,5], rpn scores [B*R], cls_prob [B*R,K], bbox_pred [B*R,4]).  No parameter is
-        touched.  BatchNorm + clip run as one `sniper_affine_act` pass per layer (the GEMM epilogue has ReLU, not clip)."""
+        touched.  BatchNorm + clip run as one `sniper_affine_act` pass per layer (the GEMM epilogue has ReLU, not clip).
+        autofocus: the `tester.DetectionNetwork` argument; this graph has no FocusPixel branch, so True is refused."""
+        if autofocus:
+            raise RuntimeError("forward_inference(autofocus=True): the MobileNetV2 graph has no FocusPixel branch")
         cfg = self.cfg
         lowp = bool(cfg.bf16)
         for b in self.all_bns():

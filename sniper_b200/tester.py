@@ -27,6 +27,7 @@ import math
 import os
 import pickle
 import time
+from typing import Protocol
 
 import numpy as np
 import torch
@@ -37,9 +38,11 @@ from ._lib import check, lib
 
 class _ImageCanvas(object):
     """Pixel stage of the test iterators: uint8 source rectangles, resized by their scale and zero-padded into an
-    SH x SW canvas minus PIXEL_MEANS by one `sniper_chip_input_hw` launch per batch."""
+    SH x SW canvas minus PIXEL_MEANS by one `sniper_chip_input_hw` launch per batch.  The canvas geometry follows the
+    backbone's stride, config.network.RPN_FEAT_STRIDE (`_canvas_size`)."""
 
     def _init_canvas(self, config, device, image_loader):
+        self.stride = int(config.network.RPN_FEAT_STRIDE)
         self.device = torch.device(device)
         self.image_loader = image_loader
         self.on_gpu = self.device.type == "cuda"        # host-only use (tests of the batching logic): no canvas is built
@@ -87,10 +90,30 @@ class _ImageCanvas(object):
         return dict(data=data, im_info=torch.from_numpy(im_info).to(dev))
 
 
-def _canvas_size(h, w):
-    """The network needs a canvas that survives the stride-16 backbone; the conv kernel wants every layer's output width
-    to be a multiple of 8 pixels (stride 16 -> the canvas width a multiple of 128), heights are free (multiple of 32)."""
-    return -(-h // 32) * 32, -(-w // 128) * 128
+class DetectionNetwork(Protocol):
+    """What `Tester`, the test iterators and `imdb_detection_wrapper` read from a network (`model.SniperResNet101`,
+    `model_mnv2.SniperMobileNetV2`):
+
+      device             where the batches are built and the detections are kept
+      feat_stride        the backbone's output stride (16 / 32); it must equal the config's network.RPN_FEAT_STRIDE,
+                         from which the iterators size their canvases
+      af                 the FocusPixel branch, or None for a network without one (then no FocusPixel map is asked for)
+      forward_inference  (data [B,3,H,W], im_info [B,3], autofocus=False) -> (rois [B*R,5], rpn scores [B*R],
+                         cls_prob [B*R,K], bbox_pred [B*R,4], + the FocusPixel map with autofocus=True); bbox_pred is
+                         class-agnostic: every class takes its box from columns 0:4, as the reference's get_detections"""
+    device: object
+    feat_stride: int
+    af: object
+
+    def forward_inference(self, data, im_info, autofocus=False): ...
+
+
+def _canvas_size(h, w, stride=16):
+    """A canvas that survives a backbone of output stride `stride`: the conv kernel wants every layer's output width to
+    be a multiple of 8 pixels (so the canvas width a multiple of 8 * stride: 128 at stride 16, 256 at stride 32); heights
+    are free (a multiple of 32, which every stride-16 or stride-32 layer divides)."""
+    hm, wm = max(32, stride), 8 * stride
+    return -(-h // hm) * hm, -(-w // wm) * wm
 
 
 class MNIteratorTestAutoFocus(_ImageCanvas):
@@ -177,7 +200,7 @@ class MNIteratorTestAutoFocus(_ImageCanvas):
             x1, x2 = max(int(cur_chip[0]), 0), min(int(cur_chip[2]), im.shape[1])
             rects.append((im, y1, y2, x1, x2, False))
             scales.append(scale)
-        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1]))
+        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1], self.stride))
         out.update(im_ids=np.array(im_ids, dtype=int), chip_ids=local_chip_ids.astype(int), scales=np.array(scales))
         return out
 
@@ -238,13 +261,14 @@ class MNIteratorTest(_ImageCanvas):
             im = self._image(r)
             rects.append((im, 0, im.shape[0], 0, im.shape[1], bool(r.get('flipped', False))))
             scales.append(chips_inference.image_scale(r['width'], r['height'], self.test_scale))
-        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1]))
+        out = self._canvas(rects, scales, *_canvas_size(max_size[0], max_size[1], self.stride))
         out.update(im_ids=np.array(im_ids, dtype=int), scales=np.array(scales))
         return out
 
 
 class Tester(object):
-    """Tester(module, imdb, roidb, test_iter, cfg, ...): `module` = a `SniperResNet101` (forward_inference)."""
+    """Tester(module, imdb, roidb, test_iter, cfg, ...): `module` = a `DetectionNetwork` (`SniperResNet101`,
+    `SniperMobileNetV2`) for the detections, or a network with `forward_rpn` for the proposals."""
 
     def __init__(self, module, imdb, roidb, test_iter, cfg, rcnn_output_names=None, rpn_output_names=None, logger=None,
                  batch_size=None, num_classes=None):
@@ -295,8 +319,9 @@ class Tester(object):
         if want_map:
             fm = out[4].cpu().numpy()
             info = batch['im_info'].cpu().numpy()
+            s = float(self.net.feat_stride)
             for idx in range(B):       # the map of the chip itself (the canvas is padded to the batch maximum)
-                mh, mw = int(math.ceil(info[idx, 0] / 16.0)), int(math.ceil(info[idx, 1] / 16.0))
+                mh, mw = int(math.ceil(info[idx, 0] / s)), int(math.ceil(info[idx, 1] / s))
                 maps.append(fm[idx, :mh, :mw].copy())
         return scores, preds, batch, batch['im_ids'], maps, batch['chip_ids']
 
@@ -316,7 +341,8 @@ class Tester(object):
         for batch in self.test_iter:
             t0 = time.time()
             scores, boxes, _, im_ids, maps, chip_ids = self.detect(batch)
-            torch.cuda.synchronize()
+            if torch.device(self.net.device).type == "cuda":
+                torch.cuda.synchronize()
             self.detect_time += time.time() - t0
             t0 = time.time()
             for i, (cscores, cboxes, im_id, chip_id) in enumerate(zip(scores, boxes, im_ids, chip_ids)):
@@ -356,10 +382,11 @@ class Tester(object):
         dets.finish()
         self.detect_time += time.time() - t0
         t0 = time.time()
+        s = float(self.net.feat_stride)
         for fm, info, im_ids, chip_ids in staged:
             fm, info = fm.numpy(), info.numpy()
             for idx, (im_id, chip_id) in enumerate(zip(im_ids, chip_ids)):
-                mh, mw = int(math.ceil(info[idx, 0] / 16.0)), int(math.ceil(info[idx, 1] / 16.0))
+                mh, mw = int(math.ceil(info[idx, 0] / s)), int(math.ceil(info[idx, 1] / s))
                 all_maps[im_id][chip_id] = (None, fm[idx, :mh, :mw].copy())
         self.post_time += time.time() - t0
         return dets, all_maps
@@ -382,8 +409,12 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     to the soft-NMS (`Tester.get_detections(backend="device")`); stats then carry `detections_pre_nms` per scale.
     With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
     dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
-    and its seconds to stats['eval_s']."""
+    and its seconds to stats['eval_s'].  `net` is a `DetectionNetwork`; config is the network's own (e.g.
+    iterator.default_config(network="mobilenetv2") for a SniperMobileNetV2): its RPN_FEAT_STRIDE must be the net's."""
     T = config.TEST
+    if int(config.network.RPN_FEAT_STRIDE) != int(net.feat_stride):
+        raise ValueError("imdb_detection_wrapper: config.network.RPN_FEAT_STRIDE is %s, the network's stride is %s"
+                         % (config.network.RPN_FEAT_STRIDE, net.feat_stride))
     for r in roidb:
         r['inference_crops'] = np.array([[0, 0, r['width'], r['height']]])
     detections, stats = [], dict(scales=[])
