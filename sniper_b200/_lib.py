@@ -83,6 +83,8 @@ SIGNATURES = {
     "sniper_coco_box_iou_batched": ("i", "ppppppppp" "i" "pp"),
     "sniper_coco_match": ("i", "ppppppppppp" "i" "pi" "pi" "pppppp"),
     "sniper_coco_accumulate": ("i", "pppppppp" "iiii" "pi" "pi" "ppp"),
+    "sniper_voc_match": ("i", "pppppppp" "i" "pi" "ppp"),
+    "sniper_voc_accumulate": ("i", "pppp" "iii" "pi" "ppppp"),
     "sniper_train_metric_workspace_bytes": ("z", ""),
     "sniper_train_metric_accum": ("i", "pipiiii" "pipii" "pipii" "ppppp"),
 }

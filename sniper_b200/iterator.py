@@ -459,12 +459,14 @@ def synthetic_roidb(n_images, seed=0, width=1333, height=800, n_gt=(1, 20), n_pr
     return out
 
 
-def default_config(neg=True, autofocus=False, network="resnet101"):
+def default_config(neg=True, autofocus=False, network="resnet101", dataset="coco"):
     """The slice of configs/faster/sniper_res101_e2e.yml the iterator reads (:21-39, 76-101, 120-140); autofocus=True:
     TRAIN.AUTO_FOCUS of configs/faster/sniper_res101_e2e_autofocus.yml (FocusPixel labels, thresholds 5 / 64 / 90).
     network="mobilenetv2": the network and TEST blocks of configs/faster/sniper_mobilenetv2_e2e.yml instead (stride 32,
     scales 1 / 2 / 4 / 8 / 12: 15 anchors; plain multi-scale inference without AutoFocus), for
-    model_mnv2.SniperMobileNetV2."""
+    model_mnv2.SniperMobileNetV2.
+    dataset="pascal_voc" (network "resnet101"): the blocks of configs/faster/sniper_res101_e2e_pascal_voc.yml instead,
+    for a 21-class SniperResNet101 evaluated by pascal_voc.PascalVOC."""
     import types
     S = types.SimpleNamespace
     if network == "resnet101":
@@ -486,10 +488,27 @@ def default_config(neg=True, autofocus=False, network="resnet101"):
                  RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, RPN_MIN_SIZE=0)
     else:
         raise ValueError("default_config: network must be 'resnet101' or 'mobilenetv2', not %r" % (network,))
+    num_classes = 81
+    if dataset == "pascal_voc":
+        if network != "resnet101":
+            raise ValueError("default_config: the PASCAL VOC config is a ResNet-101 one, not %r" % (network,))
+        # configs/faster/sniper_res101_e2e_pascal_voc.yml: PIXEL_MEANS :17-20, the anchors :21-39, NUM_CLASSES :41;
+        # TEST :177-225 (MAX_PER_IMAGE :177, SCALES :180-183, BATCH_IMAGES :186-189, VALID_RANGES :204-207, NMS / sigma
+        # :224-225).  AUTO_FOCUS / DO_PRUNING / CHIP_HYPERPARAMS are not in the yml and keep
+        # configs/faster/default_configs.py:164-166.
+        net = S(PIXEL_MEANS=[103.939, 116.779, 123.68], ANCHOR_SCALES=[2, 4, 7, 10, 13, 16, 24], ANCHOR_RATIOS=[0.5, 1, 2],
+                RPN_FEAT_STRIDE=16, NUM_ANCHORS=21)
+        test = S(SCALES=[(1400, 2000), (800, 1280), (480, 512)], BATCH_IMAGES=[2, 2, 4], MAX_PER_IMAGE=200,
+                 VALID_RANGES=[(-1, 90), (32, 180), (75, -1)], AUTO_FOCUS=False, DO_PRUNING=[False, False, False],
+                 CHIP_HYPERPARAMS=[(-1, -1, -1), (-1, -1, -1), (-1, -1, -1)], NMS=-1, NMS_SIGMA=0.55,
+                 RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, RPN_MIN_SIZE=0)
+        num_classes = 21
+    elif dataset != "coco":
+        raise ValueError("default_config: dataset must be 'coco' or 'pascal_voc', not %r" % (dataset,))
     return S(network=net,
              TRAIN=S(SCALES=[(1400, 2000), (800, 1280), (-1, 512)], VALID_RANGES=[(-1, 80), (32, 150), (120, -1)],
                      CPP_CHIPS=True, USE_NEG_CHIPS=neg, RPN_BATCH_SIZE=256, RPN_FG_FRACTION=0.5,
                      RPN_POSITIVE_OVERLAP=0.5, RPN_NEGATIVE_OVERLAP=0.4, BATCH_IMAGES=16, AUTO_FOCUS=autofocus,
                      AUTO_FOCUS_DC_LOW=5, AUTO_FOCUS_SMALL_THRESH=64, AUTO_FOCUS_DC_HIGH=90),
              TEST=test,
-             dataset=S(NUM_CLASSES=81))
+             dataset=S(NUM_CLASSES=num_classes))

@@ -992,3 +992,62 @@ def add_rows(a, b, out=None):
     assert a.dtype == b.dtype == out.dtype and a.shape == b.shape
     check(lib().sniper_add_rows(_ptr(a), lda, _ptr(b), _rows(b)[2], _ptr(out), _rows(out)[2], M, C, _sdt(a), _stream()))
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# PASCAL VOC box evaluation (lib/dataset/pascal_voc_eval.py:73-181): detections class-major in the host's
+# np.argsort(-confidence) order, GTs a CSR over the (class, image) pairs p = c * num_images + i (host int32 offsets)
+# ---------------------------------------------------------------------------------------------
+def voc_match(det_box, det_pair, gt_box, gt_difficult, gt_off, thresholds):
+    """The matching loop of voc_eval (pascal_voc_eval.py:137-171) for every (class, image) pair and every overlap
+    threshold in one launch.  det_box: [N, 4] float64 device, the results file's boxes in sorted order; det_pair: host
+    int array [N], the pair of each sorted position; gt_box [G, 4] float64 and gt_difficult [G] uint8 device, in the
+    CSR order of gt_off (host [P+1]).  Returns flags [T, N] uint8 (1 tp, 2 fp, 0 a hit on a difficult GT)."""
+    gt_off = _off(gt_off)
+    P = gt_off.size - 1
+    thr = np.ascontiguousarray(thresholds, dtype=np.float64).reshape(-1)
+    T = thr.size
+    det_pair = np.ascontiguousarray(det_pair, dtype=np.int64).reshape(-1)
+    N, G = det_pair.size, int(gt_off[-1])
+    if N and (det_pair.min() < 0 or det_pair.max() >= P):
+        raise ValueError("voc_match: a detection's pair index is outside [0, %d)" % P)
+    if tuple(det_box.shape) != (N, 4) or tuple(gt_box.shape) != (G, 4) or tuple(gt_difficult.shape) != (G,):
+        raise ValueError("voc_match: det_box must be [N, 4], gt_box [G, 4] and gt_difficult [G] (N = %d, G = %d)"
+                         % (N, G))
+    assert gt_difficult.dtype == torch.uint8
+    # every pair's sorted positions in increasing order
+    pos = np.argsort(det_pair, kind="stable").astype(np.int32)
+    pair_off = np.zeros(P + 1, np.int32)
+    np.cumsum(np.bincount(det_pair, minlength=P), out=pair_off[1:])
+    dev = gt_box.device
+    flags = torch.empty(T, N, dtype=torch.uint8, device=dev)
+    taken = torch.empty(T, max(G, 1), dtype=torch.uint8, device=dev)
+    d_pair, d_pos, d_gt = (torch.from_numpy(a).to(dev) for a in (pair_off, pos, gt_off))
+    check(lib().sniper_voc_match(_ptr(_f64(det_box)), _ptr(d_pair), _ptr(d_pos), _ptr(_f64(gt_box)),
+                                 _ptr(gt_difficult.contiguous()), _ptr(d_gt), pair_off.ctypes.data, gt_off.ctypes.data,
+                                 P, thr.ctypes.data, T, _ptr(flags), _ptr(taken), _stream()))
+    return flags
+
+
+def voc_accumulate(flags, det_off, npos, use_07_metric, thresholds_07=None):
+    """pascal_voc_eval.py:173-179 and voc_ap (:39-70) for every class and threshold, one block each: rec and prec
+    [T, N] float64 (class c at det_off[c]:det_off[c+1], host [C+1]) and ap [T, C] float64, all on the device.  npos:
+    [C] int32 device, the non-difficult GT count of each class.  The 11-point metric takes its recall thresholds from
+    the host (default np.arange(0., 1.1, 0.1)); the area metric sums in numpy's pairwise order."""
+    det_off = _off(det_off)
+    C = det_off.size - 1
+    T, N = flags.shape
+    if int(det_off[-1]) != N:
+        raise ValueError("voc_accumulate: det_off ends at %d, flags hold %d positions" % (det_off[-1], N))
+    t07 = np.ascontiguousarray(np.arange(0., 1.1, 0.1) if thresholds_07 is None else thresholds_07, dtype=np.float64)
+    dev = flags.device
+    assert npos.dtype == torch.int32 and tuple(npos.shape) == (C,)
+    rec = torch.empty(T, N, dtype=torch.float64, device=dev)
+    prec = torch.empty(T, N, dtype=torch.float64, device=dev)
+    ap = torch.empty(T, C, dtype=torch.float64, device=dev)
+    terms = None if use_07_metric else torch.empty(T, N + C, dtype=torch.float64, device=dev)
+    d_off = torch.from_numpy(det_off).to(dev)
+    check(lib().sniper_voc_accumulate(_ptr(flags.contiguous()), _ptr(d_off), _ptr(npos.contiguous()),
+                                      det_off.ctypes.data, C, T, int(bool(use_07_metric)), t07.ctypes.data, t07.size,
+                                      _ptr(rec), _ptr(prec), _ptr(ap), _ptr(terms), _stream()))
+    return rec, prec, ap

@@ -74,6 +74,8 @@ DOC = {
     "sniper_coco_box_iou_batched": "bbIou (lib/dataset/pycocotools/maskApi.c:98-109, reached through mask.iou from COCOeval.computeIoU, cocoeval.py:163-187) for every (category, image) pair of a CSR in ONE launch: pair p's [D_p x G_p] float64 matrix at out + iou_off[p]; crowd GTs (gt_flags bit 0) take the detection's area as the union.  Bit-exact (no FMA).",
     "sniper_coco_match": "COCOeval.evaluateImg (lib/dataset/pycocotools/cocoeval.py:189-272) for every pair x area range x IoU threshold in ONE launch: GTs ignore-sorted (stable), min(t, 1-1e-10), crowd re-matching, the stop at the first ignored GT, ties to the later GT, ids (not booleans) as the matched test.  Writes dt_flags[A,T,Dtot] (bit 0 matched, bit 1 ignored), npig[P,A] and gt_match[A,T,Gtot] (matching dt id, 0 = none, in ignore-sorted order); dt_match[A,T,Dtot] (matched gt id) and gt_order[A,Gtot] (ignore-sorted GT order) only when non-null.",
     "sniper_coco_accumulate": "COCOeval.accumulate (lib/dataset/pycocotools/cocoeval.py:274-374): precision[T,R,K,A,M] and recall[T,K,A,M] float64, one block per (category, area, maxDet, threshold), from sniper_coco_match's flags and one stable (category, descending score) order of the detections (cat_order) with their in-image ranks (dt_rank).  Byte-equal to the reference, -1 where it leaves -1.",
+    "sniper_voc_match": "The matching loop of voc_eval (lib/dataset/pascal_voc_eval.py:137-171) for every (class, image) pair x overlap threshold in ONE launch, the pair's detections in the host's np.argsort(-confidence) order (:127-131): overlaps with +1 pixel extents, ovmax / jmax as np.max / np.argmax (a NaN wins, first maximum), the strict `ovmax > ovthresh`, difficult GTs neither tp nor fp, a second hit on a taken GT an fp.  flags[T,N] uint8: 1 tp, 2 fp, 0 neither; taken[T,G] is the reference's det scratch.  Bit-exact (no FMA).",
+    "sniper_voc_accumulate": "pascal_voc_eval.py:173-179 and voc_ap (:39-70) for every class x threshold, one block each: integer tp / fp scans, rec = tp / float(npos), prec = tp / max(tp + fp, eps), then the 11-point AP (host recall thresholds, ap += p / 11. in order) or the area AP (mpre envelope, terms where mrec changes summed in numpy's pairwise order; terms is [T, N + C] scratch).  rec / prec [T,N] and ap [T,C] float64, byte-equal to the reference's.",
     "sniper_train_metric_workspace_bytes": "Scratch bytes for sniper_train_metric_accum (zero-filled once by the caller; the kernel leaves it reusable).",
     "sniper_train_metric_accum": "The training metrics of lib/train_utils/metric.py:50-95, 104-300 (RPNAcc, RPNLogLoss, RPNL1Loss, RCNNAcc, RCNNLogLoss, RCNNL1LossCRCNN, AutoFocusAcc, AutoFocusLogLoss) for one step in ONE launch, added into a caller-owned accumulator (int64 num_inst[8] | int64 hits[8] | float64 sum[8]): replaces their per-step asnumpy() (:109-125).  Argmax ties to the first maximum, p + 1e-14 in float32, log and sums in float64, block partials summed in block order (byte-identical run to run).  num_inst from the step's count_valid results, the L1 sums from its loss buffer.",
     "sniper_nms_gpu":"Batched hard NMS on device for per-scale inference NMS (lib/nms/nms_kernel.cu:34-144 replacement).",
