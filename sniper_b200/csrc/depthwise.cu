@@ -47,9 +47,11 @@ int launch_fwd_tiled(const void* x, const float* w, void* y, const dwc::Params& 
   return 0;
 }
 
-// the tiled kernel takes bf16 with whole 64-channel groups; fp32 and other shapes run the register-window kernels
-bool use_tiled(int dtype, int C, long ld_in) {
-  return dtype == 1 && C % 64 == 0 && ld_in % 8 == 0;       // 16-byte aligned pixel rows for cp.async
+// the tiled kernel takes bf16 with whole 64-channel groups; fp32 and other shapes run the register-window kernels.
+// cp.async copies 16 bytes from x + pixel * ld_in + 64k + 8j: the base and the pixel rows must both be 16-byte aligned
+// (a channel slice such as big[..., 4:68] of a bf16 map is only 8-byte aligned; it runs the register kernel, same bits)
+bool use_tiled(int dtype, int C, long ld_in, const void* in) {
+  return dtype == 1 && C % 64 == 0 && ld_in % 8 == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0;
 }
 
 template <typename T>
@@ -159,13 +161,28 @@ int fill_params(dwc::Params& p, int NB, int H, int W, int C, int stride, long ld
                 const char* who) {
   SN_CHECK(dtype == 0 || dtype == 1, "%s: dtype must be 0 (fp32) or 1 (bf16)", who);
   SN_CHECK(stride == 1 || stride == 2, "%s: stride must be 1 or 2", who);
-  SN_CHECK(NB > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "%s: C (%d) must be a positive multiple of 4", who, C);
+  SN_CHECK(NB > 0 && H > 0 && W > 0, "%s: NB (%d), H (%d) and W (%d) must be positive", who, NB, H, W);
+  SN_CHECK(C > 0 && C % 4 == 0, "%s: C (%d) must be a positive multiple of 4", who, C);
   SN_CHECK(ld_in >= C && ld_out >= C && ld_in % 4 == 0 && ld_out % 4 == 0, "%s: pixel strides must be multiples of 4 and >= C",
            who);
   p.NB = NB; p.H = H; p.W = W; p.C = C; p.stride = stride;
   p.Ho = (H - 1) / stride + 1;          // (H + 2*1 - 3) / stride + 1
   p.Wo = (W - 1) / stride + 1;
   p.ldx = ld_in; p.ldy = ld_out;
+  return 0;
+}
+
+// The pointers of a forward / data-gradient launch: the map operands are read and written as 4-channel vectors (float4
+// in fp32, 8 bytes in bf16) and the weights as float4, so each must be non-null and aligned to its vector.
+int check_ptrs(const void* in, const char* in_name, const float* w, const void* out, const char* out_name, int dtype,
+               const char* who) {
+  const uintptr_t vec = dtype == 0 ? 16 : 8;
+  SN_CHECK(in != nullptr, "%s: %s must not be null", who, in_name);
+  SN_CHECK(reinterpret_cast<uintptr_t>(in) % vec == 0, "%s: %s must be %d-byte aligned", who, in_name, (int)vec);
+  SN_CHECK(w != nullptr, "%s: w must not be null", who);
+  SN_CHECK((reinterpret_cast<uintptr_t>(w) & 15) == 0, "%s: w must be 16-byte aligned", who);
+  SN_CHECK(out != nullptr, "%s: %s must not be null", who, out_name);
+  SN_CHECK(reinterpret_cast<uintptr_t>(out) % vec == 0, "%s: %s must be %d-byte aligned", who, out_name, (int)vec);
   return 0;
 }
 
@@ -176,12 +193,16 @@ inline unsigned blocks_for(long nthreads) { return (unsigned)((nthreads + kTPB -
 extern "C" {
 
 // y[NB,Ho,Wo,C] = depthwise3x3(x[NB,H,W,C], w[9,C]), pad 1, stride 1 | 2.  ldx / ldy: elements between pixels.
+// Alignment: x and y 16-byte (fp32) / 8-byte (bf16) aligned, w [9,C] fp32 16-byte aligned; refused otherwise.  bf16
+// with C % 64 == 0, ldx % 8 == 0 and a 16-byte aligned x runs the shared-memory tiled kernel, anything else the
+// register kernel; both give the same bits.
 int sniper_depthwise3x3_fwd(const void* x, long ldx, const float* w, void* y, long ldy, int NB, int H, int W, int C,
                             int stride, int dtype, void* stream) {
   dwc::Params p;
   if (fill_params(p, NB, H, W, C, stride, ldx, ldy, dtype, "depthwise3x3_fwd")) return -1;
+  if (check_ptrs(x, "x", w, y, "y", dtype, "depthwise3x3_fwd")) return -1;
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_tiled(dtype, C, ldx)) {
+  if (use_tiled(dtype, C, ldx, x)) {
     if (stride == 1 ? launch_fwd_tiled<1, false>(x, w, y, p, st) : launch_fwd_tiled<2, false>(x, w, y, p, st)) return -1;
     SN_LAUNCH_CHECK();
     return 0;
@@ -200,13 +221,16 @@ int sniper_depthwise3x3_fwd(const void* x, long ldx, const float* w, void* y, lo
 
 // dx[NB,H,W,C] = depthwise3x3^T(dy[NB,Ho,Wo,C], w[9,C]); H, W, stride describe the FORWARD convolution.
 // stride 1: the forward kernel on dy with the flipped filter; stride 2: one thread per dy pixel -> 2 x 2 block of dx.
+// Alignment as for the forward (dy in the place of x, dx in the place of y); the stride-1 gradient picks the tiled
+// kernel by the forward's rule applied to dy.
 int sniper_depthwise3x3_dgrad(const void* dy, long lddy, const float* w, void* dx, long lddx, int NB, int H, int W,
                               int C, int stride, int dtype, void* stream) {
   dwc::Params p;
   cudaStream_t st = (cudaStream_t)stream;
   if (stride == 1) {
     if (fill_params(p, NB, H, W, C, 1, lddy, lddx, dtype, "depthwise3x3_dgrad")) return -1;   // "input" = dy, "output" = dx
-    if (use_tiled(dtype, C, lddy)) {
+    if (check_ptrs(dy, "dy", w, dx, "dx", dtype, "depthwise3x3_dgrad")) return -1;
+    if (use_tiled(dtype, C, lddy, dy)) {
       if (launch_fwd_tiled<1, true>(dy, w, dx, p, st)) return -1;
       SN_LAUNCH_CHECK();
       return 0;
@@ -218,6 +242,7 @@ int sniper_depthwise3x3_dgrad(const void* dy, long lddy, const float* w, void* d
       dw_fwd_kernel<bf16, 1, 4, true><<<blocks_for(nt), kTPB, 0, st>>>(static_cast<const bf16*>(dy), w, static_cast<bf16*>(dx), p, nt);
   } else {
     if (fill_params(p, NB, H, W, C, stride, lddx, lddy, dtype, "depthwise3x3_dgrad")) return -1;
+    if (check_ptrs(dy, "dy", w, dx, "dx", dtype, "depthwise3x3_dgrad")) return -1;
     const long nt = dwc::dgrad_s2_threads(p);
     if (dtype == 0)
       dw_dgrad_s2_kernel<float><<<blocks_for(nt), kTPB, 0, st>>>(static_cast<const float*>(dy), w, static_cast<float*>(dx), p, nt);
@@ -310,12 +335,18 @@ int sniper_depthwise3x3_wgrad(const void* x, long ldx, const void* dy, long lddy
 }
 
 // col[NB*Ho*Wo, Kp] = im2col of a 3x3 / stride 2 / pad 1 convolution over an fp32 NCHW image with 3 channels, K order
-// (kh, kw, ci), zero-padded to Kp (a multiple of the wgmma kernel's K atom: 32 fp32 / 64 bf16 elements).
+// (kh, kw, ci), zero-padded to Kp (a multiple of the wgmma kernel's K atom: 32 fp32 / 64 bf16 elements).  col must be
+// 16-byte (fp32) / 8-byte (bf16) aligned: each thread stores 4 consecutive columns.
 int sniper_im2col3x3s2_nchw(const float* x, void* col, int NB, int H, int W, int Cin, int Kp, int dtype, void* stream) {
   SN_CHECK(dtype == 0 || dtype == 1, "im2col3x3s2: dtype must be 0 (fp32) or 1 (bf16)");
   SN_CHECK(Cin == 3, "im2col3x3s2: built for the 3-channel first layer (Cin = %d)", Cin);
   SN_CHECK(Kp >= 27 && Kp % 4 == 0, "im2col3x3s2: Kp (%d) must be a multiple of 4 and >= 27", Kp);
   SN_CHECK(NB > 0 && H > 0 && W > 0, "im2col3x3s2: empty input");
+  SN_CHECK(x != nullptr, "im2col3x3s2: x must not be null");
+  SN_CHECK((reinterpret_cast<uintptr_t>(x) & 3) == 0, "im2col3x3s2: x must be 4-byte aligned");
+  SN_CHECK(col != nullptr, "im2col3x3s2: col must not be null");
+  const uintptr_t vec = dtype == 0 ? 16 : 8;          // col is written as 4-column vectors
+  SN_CHECK(reinterpret_cast<uintptr_t>(col) % vec == 0, "im2col3x3s2: col must be %d-byte aligned", (int)vec);
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   const long nt = (long)NB * Ho * Wo * (Kp >> 2);
   cudaStream_t st = (cudaStream_t)stream;

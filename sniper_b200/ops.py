@@ -919,28 +919,30 @@ def coco_accumulate(dt_flags, dt_rank, cat_order, dt_off, npig, cat_pair_off, ma
 # MobileNetV2 layers (symbols/faster/mobilenetv2_e2e.py): depthwise 3x3, first-layer im2col, shortcut add
 # ---------------------------------------------------------------------------------------------
 def depthwise3x3(x, w, stride=1, out=None):
-    """x: [N,H,W,C] (fp32 | bf16), w: [9,C] fp32 tap-major -> [N,Ho,Wo,C]; pad 1."""
+    """x: [N,H,W,C] (fp32 | bf16), w: [9,C] fp32 tap-major -> [N,Ho,Wo,C]; pad 1.  x and out may be channel slices."""
     NB, H, W, C = x.shape
-    assert w.shape == (9, C) and w.dtype == torch.float32 and w.is_contiguous() and x.stride(3) == 1
-    ldx = x.stride(2)
-    assert x.stride(1) == W * ldx and x.stride(0) == H * W * ldx
+    assert w.shape == (9, C) and w.dtype == torch.float32 and w.is_contiguous()
+    ldx = _pixel_ld(x)
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     if out is None:
         out = torch.empty(NB, Ho, Wo, C, device=x.device, dtype=x.dtype)
     assert out.dtype == x.dtype and out.shape == (NB, Ho, Wo, C)
-    check(lib().sniper_depthwise3x3_fwd(_ptr(x), ldx, _ptr(w), _ptr(out), out.stride(2), NB, H, W, C, stride, _sdt(x),
+    check(lib().sniper_depthwise3x3_fwd(_ptr(x), ldx, _ptr(w), _ptr(out), _pixel_ld(out), NB, H, W, C, stride, _sdt(x),
                                         _stream()))
     return out
 
 
 def depthwise3x3_dgrad(dy, w, in_hw, stride=1, out=None):
-    """dx [N,H,W,C] of depthwise3x3 for dy [N,Ho,Wo,C]."""
+    """dx [N,H,W,C] of depthwise3x3 for dy [N,Ho,Wo,C].  dy and out may be channel slices."""
     NB, Ho, Wo, C = dy.shape
     H, W = in_hw
-    assert (H - 1) // stride + 1 == Ho and (W - 1) // stride + 1 == Wo and dy.is_contiguous()
+    assert (H - 1) // stride + 1 == Ho and (W - 1) // stride + 1 == Wo
+    assert w.shape == (9, C) and w.dtype == torch.float32 and w.is_contiguous()
+    lddy = _pixel_ld(dy)
     if out is None:
         out = torch.empty(NB, H, W, C, device=dy.device, dtype=dy.dtype)
-    check(lib().sniper_depthwise3x3_dgrad(_ptr(dy), dy.stride(2), _ptr(w), _ptr(out), out.stride(2), NB, H, W, C, stride,
+    assert out.dtype == dy.dtype and out.shape == (NB, H, W, C)
+    check(lib().sniper_depthwise3x3_dgrad(_ptr(dy), lddy, _ptr(w), _ptr(out), _pixel_ld(out), NB, H, W, C, stride,
                                           _sdt(dy), _stream()))
     return out
 
@@ -981,6 +983,7 @@ def im2col3x3s2(x_nchw, Kp, dtype=torch.float32, out=None):
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
     if out is None:
         out = torch.empty(NB, Ho, Wo, Kp, device=x_nchw.device, dtype=dtype)
+    assert out.shape == (NB, Ho, Wo, Kp) and out.is_contiguous()
     check(lib().sniper_im2col3x3s2_nchw(_ptr(x_nchw), _ptr(out), NB, H, W, Cin, Kp, _sdt(out), _stream()))
     return out
 

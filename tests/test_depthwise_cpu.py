@@ -1,7 +1,7 @@
 """The per-thread bodies of the depthwise kernels (sniper_b200/csrc/depthwise_core.cuh) executed on the CPU by
 tests/dw_emulate.cu with the launch geometry of depthwise.cu, against torch float64 (grouped conv2d and its autograd):
 pins the tap algebra, strides, borders, ragged widths, row strides and the weight-gradient grid decomposition without
-a GPU.  (The launches themselves are covered by tests/test_zz_mobilenet_gpu.py.)"""
+a GPU.  (The launches themselves are covered by tests/test_dw_exact_gpu.py and tests/test_dw_wgrad_exact_gpu.py.)"""
 import ctypes
 import os
 import shutil
