@@ -32,6 +32,8 @@ SIGNATURES = {
     "sniper_gemm_set_tail_workspace": ("i", "pzi"),
     "sniper_conv2d_nhwc": ("i", "pliiii" "pii" "pp" "iii" "pl" "iiiii" "i" "ppp" "l" "iii" "pp"),
     "sniper_conv2d_wgrad_nhwc": ("i", "plpl" "iiiii" "i" "pp" "iii" "p" "ii" "p"),
+    "sniper_conv2d_wgrad_scratch_bytes": ("z", "iiiii" "i" "pp" "iii" "i"),
+    "sniper_conv2d_wgrad_set_scratch": ("i", "pzip"),
     "sniper_affine_act": ("i", "plpppl" "l" "iii" "p"),
     "sniper_bn_stats": ("i", "pllippffipppppppip"),
     "sniper_bn_finalize": ("i", "plippffippppppp"),
@@ -99,6 +101,10 @@ KERNELS_PER_CALL = {
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
     "sniper_depthwise3x3_wgrad_workspace_bytes": 0, "sniper_depthwise3x3_set_wgrad_workspace": 0,
     "sniper_depthwise3x3_wgrad": 2,
+    # the operand copy kernel + the wgmma kernel of tf32 3 x 3 layers; other calls launch only the latter (counted as 2
+    # here as well)
+    "sniper_conv2d_wgrad_nhwc": 2,
+    "sniper_conv2d_wgrad_scratch_bytes": 0, "sniper_conv2d_wgrad_set_scratch": 0,
 }
 launches = [0]
 

@@ -14,10 +14,12 @@
 //   mode 0  GEMM    C[M,N]  = A[M,K] * B[N,K]^T             A,B K-major
 //   mode 1  CONV    C[pix,N] = sum_taps A[n,h+dh,w+dw,c] * B[N,(tap,c)]   A 4-D NHWC, K-major; TMA zero
 //                   fill implements padding, elementStrides implement stride
-//   mode 2  WGRAD   C[Co,(tap,ci)] += sum_pix dY[pix,Co] * X[n,h+dh,w+dw,ci]   both MN-major, split-K.  bf16:
-//                   wgmma reads the MN-major tiles directly (transpose bits); tf32 (wgmma takes K-major tf32 only):
-//                   the consumers transpose each ring stage into a second, K-major ring while the wgmma of the
-//                   previous stage run
+//   mode 2  WGRAD   C[Co,(tap,ci)] += sum_pix dY[pix,Co] * X[n,h+dh,w+dw,ci]   split-K.  bf16: both operands
+//                   MN-major, wgmma reads the tiles directly (transpose bits).  tf32 (wgmma takes K-major tf32 only),
+//                   stride-1 multi-tap layers over rows of Wo % 32 == 0 pixels: a copy kernel first writes dY^T and X^T
+//                   channel-major into the stream's scratch and the TMA loads those K-major (see WgradFeed); other
+//                   layers (wg_xpose): the consumers transpose each MN-major ring stage into a second, K-major ring
+//                   while the wgmma of the previous stage run
 //
 // The tile width BN is a template parameter, so each compiled mainloop issues one wgmma shape (4 per k-block, one
 // commit group).  The column pieces of a tail tile (PN columns) run a second, separately instantiated mainloop and
@@ -26,6 +28,8 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
+
+#include <algorithm>
 
 namespace {
 
@@ -36,7 +40,7 @@ constexpr int kStageABytes = 128 * 128;  // 128 rows x 128 B
 constexpr int kStatsBytes = 8 * 2 * 256 * 4;   // per-warp column sums / sums of squares (fused BatchNorm statistics)
 constexpr int kThreads = 384;            // producer warpgroup + 2 consumer warpgroups
 constexpr int kMmasPerKb = 4;            // a k-block is 128 B of K per row: 4 x k8 (tf32) / k16 (bf16) wgmma
-constexpr int kXStages = 2;              // tf32 WGRAD: stages of the K-major ring the consumers transpose into
+constexpr int kXStages = 2;              // tf32 WGRAD, wg_xpose: stages of the K-major ring the consumers transpose into
 
 struct GemmParams {
   int mode, dtype;
@@ -57,6 +61,11 @@ struct GemmParams {
   int Ho, Wo;             // output spatial extent (CONV/WGRAD pixel space)
   int kp;                 // WGRAD: pixels per k-block
   int wg_cin_blocks;      // WGRAD: N tiles per tap = Cin / block_n
+  // tf32 WGRAD from the channel-major copies (WgradFeed): X^T row block of each tap, input rows padded to wg_hp with
+  // wg_padh of them before the first
+  int wg_hp, wg_padh;
+  int wg_tapblk[kMaxTaps];
+  int wg_xpose;           // tf32 WGRAD without copies: MN-major boxes, transposed by the consumers
   // ---- descriptors (16-byte units)
   uint32_t a_lbo, a_sbo, b_lbo, b_sbo;
   uint32_t a_kadv, b_kadv;              // per wgmma k-step
@@ -308,9 +317,9 @@ __device__ __forceinline__ void xpose_next(const Ring& raw, int& rs, uint32_t& r
 }
 
 // One work unit of W output columns (W = BN for a whole tile, PN for a column piece): mainloop, split-K parking and
-// epilogue.  s / ph: position in the ring, carried across units.  XP (tf32 weight gradient): the consumers read the
-// K-major ring and fill it themselves from the TMA ring (raw, position rs / rph): the transpose of stage i + 1 runs while
-// the tensor cores work on the wgmma of stage i.
+// epilogue.  s / ph: position in the ring, carried across units.  XP (tf32 weight gradient kernels) with p.wg_xpose:
+// the consumers read the K-major ring and fill it themselves from the TMA ring (raw, position rs / rph): the transpose
+// of stage i + 1 runs while the tensor cores work on the wgmma of stage i.
 template <int DT, int TR, int W, bool XP>
 __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoord& tc, const Ring& ring, int& s,
                                              uint32_t& ph, const Ring& raw, int& rs, uint32_t& rph, float* st_buf,
@@ -324,9 +333,8 @@ __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoor
   float acc[W / 2];
 #pragma unroll
   for (int i = 0; i < W / 2; ++i) acc[i] = 0.f;
-  if constexpr (XP) {
-    if (tc.nkb > 0) xpose_next<W>(raw, rs, rph, ring, s, ph);
-  }
+  const bool xp = XP && p.wg_xpose;
+  if (xp && tc.nkb > 0) xpose_next<W>(raw, rs, rph, ring, s, ph);
   for (int i = 0; i < tc.nkb; ++i) {
     mbar_wait(&ring.full[s], ph);
     const uint32_t sa = smem_u32(ring.base + (size_t)s * ring.stride);
@@ -342,9 +350,7 @@ __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoor
     wgmma_wait<1>();
     if (i > 0 && lane == 0) mbar_arrive(&ring.empty[s == 0 ? ring.n - 1 : s - 1]);
     if (++s == ring.n) { s = 0; ph ^= 1u; }
-    if constexpr (XP) {
-      if (i + 1 < tc.nkb) xpose_next<W>(raw, rs, rph, ring, s, ph);
-    }
+    if (xp && i + 1 < tc.nkb) xpose_next<W>(raw, rs, rph, ring, s, ph);
   }
   wgmma_wait<0>();
   if (tc.nkb > 0 && lane == 0) mbar_arrive(&ring.empty[s == 0 ? ring.n - 1 : s - 1]);
@@ -367,12 +373,16 @@ __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoor
     if (old != nsl - 1) return;          // another slice finishes this tile
     if (ct == 0) p.tail_cnt[tc.tail] = 0;       // self-cleaning for the next launch
     __threadfence();
+    // slice by slice, each slice's W / 2 loads independent of one another: a loop over the slices inside the loop over
+    // the elements waited out one L2 round trip per load (nsl * W / 2 of them in a row, ~0.15 ms at 16 splits).  Every
+    // element is still summed in split order from slice 0, so the result is unchanged bit for bit.
     const float* src = ws + base;
 #pragma unroll
-    for (int i = 0; i < W / 2; ++i) {
-      float a = __ldcg(src + (size_t)i * 256);
-      for (int sl = 1; sl < nsl; ++sl) a += __ldcg(src + (size_t)sl * slice_elems + (size_t)i * 256);
-      acc[i] = a;
+    for (int i = 0; i < W / 2; ++i) acc[i] = __ldcg(src + (size_t)i * 256);
+    for (int sl = 1; sl < nsl; ++sl) {
+      const float* part = src + (size_t)sl * slice_elems;
+#pragma unroll
+      for (int i = 0; i < W / 2; ++i) acc[i] += __ldcg(part + (size_t)i * 256);
     }
   }
 
@@ -515,25 +525,27 @@ __device__ __forceinline__ void consume_unit(const GemmParams& p, const TileCoor
 
 // Persistent: each CTA walks work units blockIdx.x, blockIdx.x + gridDim.x, ...; the shared-memory ring runs across
 // tile boundaries, so the producer loads the next tile's operands while the consumers run this tile's epilogue.
-// MN = 1: WGRAD operands (MN-major).  BN: tile width; PN: width of a tail tile's column pieces (0: no pieces).
+// MN = 1: WGRAD operands (MN-major, or K-major copies in tf32, see WgradFeed).  BN: tile width; PN: width of a tail
+// tile's column pieces (0: no pieces).
 template <int DT, int MN, int BN, int PN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const __grid_constant__ CUtensorMap tma_bp, const __grid_constant__ GemmParams p) {
-  constexpr bool kXpose = MN == 1 && DT == DT_TF32;
+  constexpr bool kXposeOk = MN == 1 && DT == DT_TF32;
+  const bool xpose = kXposeOk && p.wg_xpose;
   constexpr uint32_t kStageBytes = kStageABytes + BN * 128u;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages x (A 16KB | B BN*128B)] | [tf32 WGRAD: kXStages K-major stages] | statistics 16 KB | barriers
+  // carve: [stages x (A 16KB | B BN*128B)] | [wg_xpose: kXStages K-major stages] | statistics 16 KB | barriers
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* xbuf = smem + (size_t)p.stages * kStageBytes;
-  float* st_buf = reinterpret_cast<float*>(xbuf + (kXpose ? kXStages * kStageBytes : 0u));
+  float* st_buf = reinterpret_cast<float*>(xbuf + (xpose ? kXStages * kStageBytes : 0u));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(st_buf) + kStatsBytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* xfull_bar = empty_bar + p.stages;     // K-major ring of a tf32 weight gradient
+  uint64_t* xfull_bar = empty_bar + p.stages;     // K-major ring of wg_xpose
   uint64_t* xempty_bar = xfull_bar + kXStages;
   int* bcast = reinterpret_cast<int*>(xempty_bar + kXStages);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int total_whole = p.tiles_m * p.tiles_n * p.splits;
   const int tail_mult = p.tail_p > 0 ? p.tail_p : 1;
   const int total_units = p.tail_first + (total_whole - p.tail_first) * tail_mult;
@@ -546,7 +558,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
     }
-    if (kXpose) {
+    if (xpose) {
       for (int s = 0; s < kXStages; ++s) {
         mbar_init(&xfull_bar[s], 8);
         mbar_init(&xempty_bar[s], 8);
@@ -597,8 +609,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             tma_load_4d(sa, &tma_a, &full_bar[s], cb * E, ow0 * p.conv_stride + p.tap_dw[tap],
                         oh0 * p.conv_stride + p.tap_dh[tap], n_img);
             tma_load_4d(sb, tc.piece ? &tma_bp : &tma_b, &full_bar[s], kb * E, tc.col0, 0, 0);
+          } else if (DT == DT_TF32 && !p.wg_xpose) {
+            // WGRAD from the K-major copies: k-block = kp = 32 consecutive output pixels = one 128-byte row of dY^T
+            // (A: 128 output channels) and of X^T (B: BN rows of one tap)
+            mbar_expect_tx(&full_bar[s], p.stage_tx_bytes);
+            const int pix0 = kb * p.kp;
+            tma_load_4d(sa, &tma_a, &full_bar[s], pix0, tc.tile_m * 128, 0, 0);
+            // the TMA takes 16-byte aligned starts along a map's first dimension: the pixel coordinate stays a multiple
+            // of 32, the tap's column offset is its row block
+            const int img = pix0 / (p.Ho * p.Wo);
+            const int rem = pix0 - img * (p.Ho * p.Wo);
+            const int oh = rem / p.Wo, ow = rem - oh * p.Wo;
+            const int xpix = (img * p.wg_hp + oh + p.tap_dh[wg_tap] + p.wg_padh) * p.Wo + ow;
+            tma_load_4d(sb, &tma_b, &full_bar[s], xpix, p.wg_tapblk[wg_tap] * p.wg_cin_blocks * p.block_n + wg_ci0, 0, 0);
           } else {
-            // WGRAD: k-block = kp consecutive output pixels of one image row block
+            // bf16 / wg_xpose WGRAD: k-block = kp consecutive output pixels of one image row block, MN-major boxes
             mbar_expect_tx(&full_bar[s], p.stage_tx_bytes);
             const int pix0 = kb * p.kp;
             const int img = pix0 / (p.Ho * p.Wo);
@@ -620,8 +645,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   // =============================== consumers: warpgroup g = 0 / 1 owns rows 64 g .. 64 g + 63 of the tile
   setmaxnreg_inc<232>();
   const Ring raw{smem, kStageBytes, p.stages, full_bar, empty_bar};
-  const Ring ring = kXpose ? Ring{xbuf, kStageBytes, kXStages, xfull_bar, xempty_bar} : raw;
-  constexpr int kTR = kXpose ? 0 : MN;
+  const Ring ring = xpose ? Ring{xbuf, kStageBytes, kXStages, xfull_bar, xempty_bar} : raw;
+  constexpr int kTR = DT == DT_TF32 ? 0 : MN;    // tf32 weight gradients are consumed K-major
   int s = 0, rs = 0;
   uint32_t ph = 0, rph = 0;
   for (int t = blockIdx.x; t < total_units; t += gridDim.x) {
@@ -632,7 +657,70 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         continue;
       }
     }
-    consume_unit<DT, kTR, BN, kXpose>(p, tc, ring, s, ph, raw, rs, rph, st_buf, bcast);
+    consume_unit<DT, kTR, BN, kXposeOk>(p, tc, ring, s, ph, raw, rs, rph, st_buf, bcast);
+  }
+}
+
+// ---------------------------------------------------------------- tf32 weight gradient: channel-major operand copies
+// dst[t * C + c, p] = src[n, oh + dh[t], ow + dw[t], c] for pixel p = (n, oh, ow) of an NB x Ho x Wo grid, zero outside
+// the map: the fp32 bits unchanged.  dY^T is the identity gather (one tap, H = Ho, W = Wo).
+struct XposeJob {
+  const float* src;
+  long ld;                // source pixel row stride (elements)
+  float* dst;
+  long pitch;             // destination row stride (elements, a multiple of 4)
+  int C;                  // channels per tap (a multiple of 32)
+  int rows;               // destination rows = taps * C (X^T: one tap per row block)
+  int P;                  // destination pixels = NB * Ho * Wo
+  int H, W, Ho, Wo;
+  int dh[kMaxTaps], dw[kMaxTaps];
+};
+struct XposeParams {
+  XposeJob job[2];        // dY^T, X^T
+  int split;              // blockIdx.y < split: 32-row blocks of job 0
+};
+
+constexpr int kXpPix = 64;   // pixels per copy block; channel rows per block: 32
+
+// 256 threads per 32 rows x 64 pixels: 16-byte loads along channels (8 lanes read one pixel's 128 B), 16-byte stores
+// along pixels (16 lanes write one row's 256 B)
+__global__ void __launch_bounds__(256) wgrad_xpose_kernel(const __grid_constant__ XposeParams xp) {
+  __shared__ __align__(16) float tile[32][kXpPix + 4];
+  int rb = blockIdx.y;
+  const XposeJob& j = rb < xp.split ? xp.job[0] : xp.job[1];
+  if (rb >= xp.split) rb -= xp.split;
+  const int p0 = blockIdx.x * kXpPix;
+  if (p0 >= j.P) return;
+  const int row0 = rb * 32;
+  const int t = row0 / j.C, c0 = row0 - t * j.C;
+  const int hw = j.Ho * j.Wo;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = threadIdx.x + 256 * r;
+    const int pl = i >> 3, q = i & 7;
+    const int pix = p0 + pl;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (pix < j.P) {
+      const int n = pix / hw, rem = pix - n * hw;
+      const int oh = rem / j.Wo, ow = rem - oh * j.Wo;
+      const int ih = oh + j.dh[t], iw = ow + j.dw[t];
+      if (ih >= 0 && ih < j.H && iw >= 0 && iw < j.W)
+        v = __ldg(reinterpret_cast<const float4*>(j.src + (((long)n * j.H + ih) * j.W + iw) * j.ld + c0 + 4 * q));
+    }
+    tile[4 * q + 0][pl] = v.x;
+    tile[4 * q + 1][pl] = v.y;
+    tile[4 * q + 2][pl] = v.z;
+    tile[4 * q + 3][pl] = v.w;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = threadIdx.x + 256 * r;
+    const int row = i >> 4, pq = 4 * (i & 15);
+    // pixels P..pitch-1 of a row are padding (never read through the TMA maps): a ragged last quad may write them
+    if (p0 + pq < j.P)
+      *reinterpret_cast<float4*>(j.dst + (long)(row0 + row) * j.pitch + p0 + pq) =
+          *reinterpret_cast<const float4*>(&tile[row][pq]);
   }
 }
 
@@ -677,11 +765,11 @@ int make_map(CUtensorMap* m, int dtype, const void* base, const uint64_t dims[4]
 constexpr int kSmemMax = 227 * 1024;       // opt-in dynamic shared memory per block (H100)
 constexpr int kSmemFixed = 1024 + kStatsBytes + 512;   // alignment slack, statistics, barriers
 
-// one persistent CTA per SM: fill shared memory with the operand ring (tf32 weight gradients also keep kXStages
+// one persistent CTA per SM: fill shared memory with the operand ring (wg_xpose weight gradients also keep kXStages
 // K-major stages for the transposed operands; at block_n = 256 that leaves a 2-stage TMA ring)
 int pick_stages(int block_n, int xpose = 0) {
   const int stage = kStageABytes + block_n * 128;
-  int s = (kSmemMax - kSmemFixed) / stage - (xpose ? kXStages : 0);
+  const int s = (kSmemMax - kSmemFixed) / stage - (xpose ? kXStages : 0);
   return s > 8 ? 8 : s;
 }
 
@@ -769,8 +857,7 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, GemmParams& p, dim3 til
     if (make_map(&mbp, p.dtype, bop->ptr, d, st, b, ones)) return -1;
   }
   if (p.tail_p > 0) units = p.tail_first + (units - p.tail_first) * p.tail_p;
-  const int xpose = (p.mode == MODE_WGRAD && p.dtype == DT_TF32) ? 1 : 0;
-  const size_t smem = smem_bytes(p.stages, p.block_n, xpose);
+  const size_t smem = smem_bytes(p.stages, p.block_n, p.wg_xpose);
   typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmParams);
   // every instantiation: operand type, MN-major operands, tile width, column-piece width (tail splits of 256-wide
   // K-major tiles only)
@@ -830,6 +917,69 @@ void fill_kmajor(GemmParams& p, int dtype, int block_n) {
   p.stage_tx_bytes = kStageABytes + p.b_box_bytes;
   p.stages = pick_stages(block_n);
 }
+
+// tf32 weight gradient operand feed.  wgmma reads tf32 K-major only and both operands are pixel-major.  For stride-1
+// layers with several taps whose output rows are Wo % 32 == 0 pixels (the 3 x 3 layers of the ResNet-101 step), a copy
+// kernel first writes them channel-major into the stream's scratch:
+//   dY^T [Cout, P], P = NB * Ho * Wo output pixels in k-block order;
+//   X^T  [cols * Cin, NB * Hp * Wo]: one row block per distinct column offset dw of the taps, X^T[j * Cin + ci,
+//        (n, hp, ow)] = X[n, hp - padh, ow + dw_j, ci] over the input rows zero-padded to Hp (padh before the first), so
+//        that tap (dh, dw_j) of the k-block at (n, oh, ow) is the 32 pixels from (n, oh + dh + padh, ow) of row block j.
+// Both are read through 2-D maps {pixels, rows} with boxes of 32 pixels x 128 / BN rows at pixel coordinates that are
+// multiples of 32 (the TMA needs 16-byte aligned starts along the first dimension, which rules out shifting a box by
+// dw).  Row pitches are rounded up to 16 bytes.  The k-block composition (32 consecutive output pixels, wgmma k-step j
+// covering pixels 8 j .. 8 j + 7) is that of the transposing path, so both give the same bits.  Other layers keep the
+// in-kernel transpose (wg_xpose): for 1 x 1 layers the copies' HBM traffic measured slower than the transpose, and a
+// tap-gathered copy (taps x the input bytes) left the stride-2 layers of the ResNet-101 step no faster and slowed the
+// MobileNetV2 step, whose RPN 3 x 3 runs on a 16-pixel-wide map.
+struct WgradFeed {
+  int padh, hp;               // zero rows before the first input row, padded height
+  int blocks;                 // row blocks of Cin rows: distinct dw
+  int blk_dw[kMaxTaps];       // column offset of each row block
+  int tapblk[kMaxTaps];       // row block each tap reads
+  long x_pixels;              // pixels per X^T row
+  long p_pitch, x_pitch;      // elements per row of dY^T / X^T
+  size_t xt_off, bytes;       // X^T offset in the scratch (256-byte aligned), total bytes
+};
+
+bool wgrad_copies(int dtype, int ntaps, int stride, int Wo) {
+  return dtype == DT_TF32 && ntaps > 1 && stride == 1 && Wo % 32 == 0;
+}
+
+WgradFeed wgrad_feed(int NB, int H, int Cin, int Cout, int ntaps, const int* tap_dh, const int* tap_dw, int Ho,
+                     int Wo) {
+  WgradFeed f;
+  memset(&f, 0, sizeof(f));
+  const long P = (long)NB * Ho * Wo;
+  int lo = 0, hi = 0;
+  for (int t = 0; t < ntaps; ++t) {
+    lo = std::max(lo, -tap_dh[t]);
+    hi = std::max(hi, Ho - 1 + tap_dh[t] - (H - 1));
+    int j = 0;
+    while (j < f.blocks && f.blk_dw[j] != tap_dw[t]) ++j;
+    if (j == f.blocks) f.blk_dw[f.blocks++] = tap_dw[t];
+    f.tapblk[t] = j;
+  }
+  f.padh = lo;
+  f.hp = H + lo + hi;
+  f.x_pixels = (long)NB * f.hp * Wo;
+  f.p_pitch = (P + 3) / 4 * 4;
+  f.x_pitch = (f.x_pixels + 3) / 4 * 4;
+  f.xt_off = ((size_t)Cout * f.p_pitch * 4 + 255) / 256 * 256;
+  f.bytes = f.xt_off + (size_t)f.blocks * Cin * f.x_pitch * 4;
+  return f;
+}
+
+// caller-owned scratch per (device, stream) (sniper_conv2d_wgrad_set_scratch); the library never allocates
+struct WgScratch {
+  int device;
+  cudaStream_t stream;
+  void* ptr;
+  size_t bytes;
+};
+constexpr int kWgScratchEntries = 32;
+WgScratch g_wg_scratch[kWgScratchEntries];
+int g_wg_scratch_n = 0;
 
 struct Epilogue {
   const float* scale;
@@ -970,8 +1120,11 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
   p.mode = MODE_WGRAD; p.dtype = dtype; p.block_n = bn; p.elems_per_128B = E;
   p.M = Cout; p.N = ntaps * Cin;
   const uint32_t chunk_bytes = (uint32_t)kp * 128u;
+  const bool copies = wgrad_copies(dtype, ntaps, stride, Wo);
+  p.wg_xpose = dtype == DT_TF32 && !copies;
   if (dtype == DT_TF32) {
-    // the consumers transpose each stage into K-major rows of 32 pixels (see transpose_stage_tf32)
+    // K-major stages, A = 128 dY channel rows, B = BN X channel rows, 32 pixels (128 B) each: loaded so from the
+    // channel-major copies (WgradFeed), or transposed by the consumers from MN-major boxes (see transpose_stage_tf32)
     p.a_lbo = 1; p.a_sbo = 64; p.b_lbo = 1; p.b_sbo = 64;
     p.a_kadv = 2; p.b_kadv = 2;
     p.a_half = 64 * 128;
@@ -983,10 +1136,15 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
     p.a_kadv = (16 * 128) >> 4; p.b_kadv = p.a_kadv;
     p.a_half = chunk_bytes;
   }
-  p.a_boxes = 128 / E; p.b_boxes = bn / E;
-  p.a_box_bytes = chunk_bytes; p.b_box_bytes = chunk_bytes;
-  p.stage_tx_bytes = (uint32_t)(p.a_boxes + p.b_boxes) * chunk_bytes;
-  p.stages = pick_stages(bn, dtype == DT_TF32 ? 1 : 0);
+  if (copies) {
+    p.a_boxes = 1; p.b_boxes = 1;
+    p.a_box_bytes = kStageABytes; p.b_box_bytes = (uint32_t)bn * 128u;
+  } else {
+    p.a_boxes = 128 / E; p.b_boxes = bn / E;
+    p.a_box_bytes = chunk_bytes; p.b_box_bytes = chunk_bytes;
+  }
+  p.stage_tx_bytes = (uint32_t)p.a_boxes * p.a_box_bytes + (uint32_t)p.b_boxes * p.b_box_bytes;
+  p.stages = pick_stages(bn, p.wg_xpose);
   p.ntaps = ntaps;
   for (int t = 0; t < ntaps; ++t) { p.tap_dh[t] = tap_dh[t]; p.tap_dw[t] = tap_dw[t]; }
   p.conv_stride = stride; p.Ho = Ho; p.Wo = Wo; p.kp = kp; p.wg_cin_blocks = Cin / bn;
@@ -1011,24 +1169,103 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
   }
   p.num_kb = (int)(total_kb / splits);
   p.C = dW; p.ldc = (long)ntaps * Cin; p.atomic = 1;
+  SN_CHECK(dy_ld >= Cout && x_ld >= Cin && (dy_ld * esz) % 16 == 0 && (x_ld * esz) % 16 == 0, "wgrad: bad ld");
+  const uint32_t ones[4] = {1, 1, 1, 1};
   CUtensorMap ma, mb;
-  {
-    SN_CHECK(dy_ld >= Cout && x_ld >= Cin && (dy_ld * esz) % 16 == 0 && (x_ld * esz) % 16 == 0, "wgrad: bad ld");
-    const uint64_t d[4] = {(uint64_t)Cout, (uint64_t)pixels, 1, 1};
-    const uint64_t s[3] = {(uint64_t)dy_ld * esz, (uint64_t)dy_ld * esz * pixels, (uint64_t)dy_ld * esz * pixels};
-    const uint32_t b[4] = {(uint32_t)E, (uint32_t)kp, 1, 1};
-    const uint32_t ones[4] = {1, 1, 1, 1};
-    if (make_map(&ma, dtype, dY, d, s, b, ones)) return -1;
-  }
-  {
-    const uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
-    const uint64_t s[3] = {(uint64_t)x_ld * esz, (uint64_t)x_ld * esz * W, (uint64_t)x_ld * esz * W * H};
-    const uint32_t b[4] = {(uint32_t)E, (uint32_t)(bw * stride), (uint32_t)(bh * stride), 1};
-    const uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
-    if (make_map(&mb, dtype, X, d, s, b, es)) return -1;
-  }
   dim3 grid(Cout / 128 + (Cout % 128 ? 1 : 0), ntaps * p.wg_cin_blocks, splits);
+  if (!copies) {
+    {
+      const uint64_t d[4] = {(uint64_t)Cout, (uint64_t)pixels, 1, 1};
+      const uint64_t s[3] = {(uint64_t)dy_ld * esz, (uint64_t)dy_ld * esz * pixels, (uint64_t)dy_ld * esz * pixels};
+      const uint32_t b[4] = {(uint32_t)E, (uint32_t)kp, 1, 1};
+      if (make_map(&ma, dtype, dY, d, s, b, ones)) return -1;
+    }
+    {
+      const uint64_t d[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
+      const uint64_t s[3] = {(uint64_t)x_ld * esz, (uint64_t)x_ld * esz * W, (uint64_t)x_ld * esz * W * H};
+      const uint32_t b[4] = {(uint32_t)E, (uint32_t)(bw * stride), (uint32_t)(bh * stride), 1};
+      const uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
+      if (make_map(&mb, dtype, X, d, s, b, es)) return -1;
+    }
+    return launch(ma, mb, p, grid, (cudaStream_t)stream);
+  }
+
+  // channel-major copies of both operands into the stream's scratch, then the K-major mainloop
+  SN_CHECK((reinterpret_cast<uintptr_t>(dY) & 15) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0,
+           "wgrad: dY and X must be 16-byte aligned");
+  const WgradFeed f = wgrad_feed(NB, H, Cin, Cout, ntaps, tap_dh, tap_dw, Ho, Wo);
+  int dev = -1;
+  SN_CUDA(cudaGetDevice(&dev));
+  const WgScratch* sc = nullptr;
+  for (int i = 0; i < g_wg_scratch_n; ++i)
+    if (g_wg_scratch[i].device == dev && g_wg_scratch[i].stream == (cudaStream_t)stream) sc = &g_wg_scratch[i];
+  SN_CHECK(sc != nullptr,
+           "wgrad: no tf32 operand scratch registered for device %d and this stream (sniper_conv2d_wgrad_set_scratch)",
+           dev);
+  SN_CHECK(sc->bytes >= f.bytes,
+           "wgrad: the stream's tf32 operand scratch holds %zu bytes, this call needs %zu (sniper_conv2d_wgrad_scratch_bytes)",
+           sc->bytes, f.bytes);
+  float* dyt = static_cast<float*>(sc->ptr);
+  float* xt = reinterpret_cast<float*>(static_cast<uint8_t*>(sc->ptr) + f.xt_off);
+  {
+    const uint64_t pb = (uint64_t)f.p_pitch * 4;
+    const uint64_t d[4] = {(uint64_t)pixels, (uint64_t)Cout, 1, 1};
+    const uint64_t s[3] = {pb, pb * Cout, pb * Cout};
+    const uint32_t b[4] = {(uint32_t)kp, 128, 1, 1};
+    if (make_map(&ma, dtype, dyt, d, s, b, ones)) return -1;
+  }
+  const long x_rows = (long)f.blocks * Cin;
+  {
+    const uint64_t xb = (uint64_t)f.x_pitch * 4;
+    const uint64_t d[4] = {(uint64_t)f.x_pixels, (uint64_t)x_rows, 1, 1};
+    const uint64_t s[3] = {xb, xb * x_rows, xb * x_rows};
+    const uint32_t b[4] = {(uint32_t)kp, (uint32_t)bn, 1, 1};
+    if (make_map(&mb, dtype, xt, d, s, b, ones)) return -1;
+  }
+  p.wg_hp = f.hp; p.wg_padh = f.padh;
+  for (int t = 0; t < ntaps; ++t) p.wg_tapblk[t] = f.tapblk[t];
+  XposeParams xp;
+  memset(&xp, 0, sizeof(xp));
+  xp.job[0] = XposeJob{static_cast<const float*>(dY), dy_ld, dyt, f.p_pitch, Cout, Cout, (int)pixels, Ho, Wo, Ho, Wo};
+  // X^T row block j: a gather over the Hp x Wo grid with offsets (-padh, dw_j)
+  XposeJob& xj = xp.job[1];
+  xj.src = static_cast<const float*>(X); xj.ld = x_ld; xj.dst = xt; xj.pitch = f.x_pitch;
+  xj.C = Cin; xj.rows = (int)x_rows; xj.P = (int)f.x_pixels; xj.H = H; xj.W = W; xj.Ho = f.hp; xj.Wo = Wo;
+  for (int j = 0; j < f.blocks; ++j) { xj.dh[j] = -f.padh; xj.dw[j] = f.blk_dw[j]; }
+  xp.split = Cout / 32;
+  const long xpix = pixels > xj.P ? pixels : xj.P;
+  const dim3 xgrid((unsigned)sn::div_up(xpix, kXpPix), (unsigned)(xp.split + xj.rows / 32));
+  wgrad_xpose_kernel<<<xgrid, 256, 0, (cudaStream_t)stream>>>(xp);
+  SN_LAUNCH_CHECK();
   return launch(ma, mb, p, grid, (cudaStream_t)stream);
+}
+
+// Bytes of the tf32 operand scratch sniper_conv2d_wgrad_nhwc needs for a geometry (host only; 0 where the kernel reads
+// the operands in place: bf16, and tf32 layers without copies, see WgradFeed).  Same arguments as that entry point.
+size_t sniper_conv2d_wgrad_scratch_bytes(int NB, int H, int W, int Cin, int Cout, int ntaps, const int* tap_dh,
+                                         const int* tap_dw, int stride, int Ho, int Wo, int dtype) {
+  if (!wgrad_copies(dtype, ntaps, stride, Wo) || ntaps > kMaxTaps || !tap_dh || !tap_dw) return 0;
+  return wgrad_feed(NB, H, Cin, Cout, ntaps, tap_dh, tap_dw, Ho, Wo).bytes;
+}
+
+// Registers a caller-owned device buffer (256-byte aligned, no initialisation) as the tf32 operand scratch of the
+// weight gradients enqueued on `stream` of `device`; it must outlive them.  Registering again for the same (device,
+// stream) replaces the buffer.  The library itself never allocates.
+int sniper_conv2d_wgrad_set_scratch(void* ptr, size_t bytes, int device, void* stream) {
+  SN_CHECK(device >= 0, "conv2d_wgrad_set_scratch: device (%d) must be >= 0", device);
+  SN_CHECK(ptr != nullptr, "conv2d_wgrad_set_scratch: ptr must not be null");
+  SN_CHECK((reinterpret_cast<uintptr_t>(ptr) & 255) == 0, "conv2d_wgrad_set_scratch: ptr must be 256-byte aligned");
+  const cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < g_wg_scratch_n; ++i)
+    if (g_wg_scratch[i].device == device && g_wg_scratch[i].stream == st) {
+      g_wg_scratch[i].ptr = ptr;
+      g_wg_scratch[i].bytes = bytes;
+      return 0;
+    }
+  SN_CHECK(g_wg_scratch_n < kWgScratchEntries, "conv2d_wgrad_set_scratch: more than %d (device, stream) pairs",
+           kWgScratchEntries);
+  g_wg_scratch[g_wg_scratch_n++] = WgScratch{device, st, ptr, bytes};
+  return 0;
 }
 
 // Bytes sniper_gemm_set_tail_workspace expects (per device).

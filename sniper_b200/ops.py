@@ -317,6 +317,29 @@ def _pixel_ld(t):
     return ld
 
 
+_wg_scratch = {}
+_wg_scratch_replaced = []
+
+
+def _ensure_wgrad_scratch(nbytes):
+    """The tf32 weight gradient copies its operands channel-major into a caller-owned scratch (the library never
+    allocates): one buffer per (device, stream), because launches on different streams may overlap, grown to the next
+    power of two when a call needs more.  A replaced buffer is kept alive for the life of the process, because a
+    captured CUDA graph may still hold its address."""
+    if nbytes == 0:
+        return
+    idx, st = torch.cuda.current_device(), _stream()
+    cur = _wg_scratch.get((idx, st))
+    if cur is not None and cur.numel() >= nbytes:
+        return
+    n = 1 << (nbytes - 1).bit_length()
+    buf = torch.empty(n, dtype=torch.uint8, device=torch.device("cuda", idx))
+    check(lib().sniper_conv2d_wgrad_set_scratch(buf.data_ptr(), n, idx, st))
+    if cur is not None:
+        _wg_scratch_replaced.append(cur)
+    _wg_scratch[(idx, st)] = buf
+
+
 def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, splits=8, taps=None):
     """dW[Cout, kh*kw*Cin] += dY^T * im2col(X).  dy: [N,Ho,Wo,Cout], x: [N,H,W,Cin]."""
     NB, H, W, Cin = x.shape
@@ -332,6 +355,8 @@ def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, spl
         "dw_out must be a contiguous fp32 [Cout, taps * Cin]"
     _, dhp = _iarr(dh)
     _, dwp = _iarr(dw)
+    _ensure_wgrad_scratch(lib().sniper_conv2d_wgrad_scratch_bytes(NB, H, W, Cin, Cout, ntaps, dhp, dwp, stride, Ho, Wo,
+                                                                   _dt(x)))
     check(lib().sniper_conv2d_wgrad_nhwc(_ptr(dy), dy_ld, _ptr(x), x_ld, NB, H, W, Cin, Cout, ntaps, dhp,
                                          dwp, stride, Ho, Wo,
                                          _ptr(dw_out), _dt(x), splits, _stream()))

@@ -24,7 +24,9 @@ DOC = {
     "sniper_gemm_tail_workspace_bytes": "Size of the caller-owned scratch the wgmma kernel's split-K weight gradient uses (per device).",
     "sniper_gemm_set_tail_workspace": "Registers that scratch (zero-filled, caller-owned, must outlive later launches); the library itself never allocates device memory.",
     "sniper_conv2d_nhwc": "NHWC implicit-GEMM convolution on wgmma; also the stride-1/stride-2 data gradient (flipped / parity-split weights, strided output map). Replaces cudnnConvolutionForward / BackwardData (nn/cudnn/cudnn_convolution-inl.h:144,211-266).",
-    "sniper_conv2d_wgrad_nhwc": "Weight gradient dW[Cout, taps*Cin] += dY^T * im2col(X) on wgmma with MN-major operands and split-K. Replaces cudnnConvolutionBackwardFilter (nn/cudnn/cudnn_convolution-inl.h:211-266).",
+    "sniper_conv2d_wgrad_nhwc": "Weight gradient dW[Cout, taps*Cin] += dY^T * im2col(X) on wgmma with split-K: bf16 reads the MN-major operands in place, tf32 first copies them channel-major into the stream's registered scratch (sniper_conv2d_wgrad_set_scratch; refused without one). Replaces cudnnConvolutionBackwardFilter (nn/cudnn/cudnn_convolution-inl.h:211-266).",
+    "sniper_conv2d_wgrad_scratch_bytes": "Host-only: bytes of the tf32 operand scratch sniper_conv2d_wgrad_nhwc needs for a geometry (0 for bf16).",
+    "sniper_conv2d_wgrad_set_scratch": "Registers that scratch (caller-owned, 256-byte aligned, no initialisation, must outlive later launches) for the weight gradients on one (device, stream); registering again replaces it. The library itself never allocates device memory.",
     "sniper_affine_act": "y = act(x*scale[c] + shift[c]) on [M,C] rows (BatchNorm apply + Activation; nn/batch_norm.cu:658-700); relu 0 = none, 1 = ReLU, 2 = clip(y, 0, 6).",
     "sniper_bn_stats": "Train-mode BatchNorm statistics -> mean, invstd, scale, shift and moving statistics (cuDNN convention, nn/cudnn/cudnn_batch_norm-inl.h).",
     "sniper_bn_apply_train": "BatchNorm(train) + Activation in one launch when the input statistics were accumulated by the producing conv's epilogue: finalisation (mean / invstd / scale / shift / moving statistics, nn/batch_norm.cu:658-700 semantics) folded into the apply pass.",
