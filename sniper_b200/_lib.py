@@ -15,6 +15,8 @@ _T = {"p": ctypes.c_void_p, "i": ctypes.c_int, "l": ctypes.c_long, "f": ctypes.c
 SIGNATURES = {
     "sniper_last_error": ("s", ""),
     "sniper_abi_version": ("i", ""),
+    "sniper_stream_workspace_bytes": ("z", ""),
+    "sniper_set_stream_workspace": ("i", "pzip"),
     "sniper_multi_proposal_target_workspace_bytes": ("z", "iiii"),
     "sniper_generate_anchors": ("i", "ipipip"),
     "sniper_proposal_decode": ("i", "pppp" "iiiii" "pipi" "iii" "ppp" "p"),
@@ -28,12 +30,9 @@ SIGNATURES = {
     "sniper_psroi_bwd": ("i", "pp" "iiii" "f" "iiii" "p" "p"),
     "sniper_gemm_nt": ("i", "plplpl" "iiii" "ppp" "l" "iii" "pp"),
     "sniper_gemm_plan": ("i", "iiiip"),
-    "sniper_gemm_tail_workspace_bytes": ("z", ""),
-    "sniper_gemm_set_tail_workspace": ("i", "pzi"),
     "sniper_conv2d_nhwc": ("i", "pliiii" "pii" "pp" "iii" "pl" "iiiii" "i" "ppp" "l" "iii" "pp"),
     "sniper_conv2d_wgrad_nhwc": ("i", "plpl" "iiiii" "i" "pp" "iii" "p" "ii" "p"),
     "sniper_conv2d_wgrad_scratch_bytes": ("z", "iiiii" "i" "pp" "iii" "i"),
-    "sniper_conv2d_wgrad_set_scratch": ("i", "pzip"),
     "sniper_affine_act": ("i", "plpppl" "l" "iii" "p"),
     "sniper_bn_stats": ("i", "pllippffipppppppip"),
     "sniper_bn_finalize": ("i", "plippffippppppp"),
@@ -44,8 +43,6 @@ SIGNATURES = {
     "sniper_affine_relu_bwd": ("i", "plplpp" "pl" "pl" "lii" "p"),
     "sniper_depthwise3x3_fwd": ("i", "plppl" "iiiiii" "p"),
     "sniper_depthwise3x3_dgrad": ("i", "plppl" "iiiiii" "p"),
-    "sniper_depthwise3x3_wgrad_workspace_bytes": ("z", ""),
-    "sniper_depthwise3x3_set_wgrad_workspace": ("i", "pzip"),
     "sniper_depthwise3x3_wgrad": ("i", "plplp" "iiiiii" "p"),
     "sniper_im2col3x3s2_nchw": ("i", "pp" "iiiiii" "p"),
     "sniper_add_rows": ("i", "plplpl" "lii" "p"),
@@ -95,16 +92,16 @@ _lib = None
 
 # GPU kernels launched per C-ABI call (host-only entry points: 0)
 KERNELS_PER_CALL = {
-    "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
+    "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_stream_workspace_bytes": 0,
+    "sniper_set_stream_workspace": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
-    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_gemm_tail_workspace_bytes": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0, "sniper_gemm_set_tail_workspace": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
+    "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
-    "sniper_depthwise3x3_wgrad_workspace_bytes": 0, "sniper_depthwise3x3_set_wgrad_workspace": 0,
     "sniper_depthwise3x3_wgrad": 2,
     # the operand copy kernel + the wgmma kernel of tf32 3 x 3 layers; other calls launch only the latter (counted as 2
     # here as well)
     "sniper_conv2d_wgrad_nhwc": 2,
-    "sniper_conv2d_wgrad_scratch_bytes": 0, "sniper_conv2d_wgrad_set_scratch": 0,
+    "sniper_conv2d_wgrad_scratch_bytes": 0,
 }
 launches = [0]
 

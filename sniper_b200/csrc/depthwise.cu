@@ -118,23 +118,6 @@ __global__ void __launch_bounds__(32 * kRdTY) dw_wgrad_reduce_kernel(const float
   }
 }
 
-// Workspace of one launch: the slab holds at most kWgSlabFloats partials.  The one-wave grid needs about
-// kNumSMs * (blocks per SM) * 9 * 128 floats (a block covers at most 128 channels); at 126..158 registers per thread
-// that is 1..2 blocks per SM, so the cap (4 blocks per SM) binds only for grids the occupancy rule would not pick.
-constexpr long kWgSlabFloats = (long)sn::kNumSMs * 4 * 9 * 128;
-
-// Caller-owned workspaces, one per (device, stream): launches on one stream run one after another and can share a
-// slab; launches on different streams may overlap and must not.  Host-side table; like the GEMM's split-K table the
-// entry points are not re-entrant across host threads (one host thread drives a device's launches).
-constexpr int kWgWsEntries = 256;
-struct WgWs {
-  int device;
-  cudaStream_t stream;
-  void* ws;
-};
-WgWs g_wg_ws[kWgWsEntries];
-int g_wg_ws_n = 0;
-
 template <typename K>
 int wgrad_blocks_per_sm(K kernel) {
   int n = 0;
@@ -253,31 +236,6 @@ int sniper_depthwise3x3_dgrad(const void* dy, long lddy, const float* w, void* d
   return 0;
 }
 
-// Bytes of the workspace sniper_depthwise3x3_set_wgrad_workspace expects (the same for every shape).
-size_t sniper_depthwise3x3_wgrad_workspace_bytes(void) { return (size_t)kWgSlabFloats * sizeof(float); }
-
-// Registers a caller-owned device buffer of sniper_depthwise3x3_wgrad_workspace_bytes() bytes (16-byte aligned, no
-// initialisation needed) for the weight-gradient launches enqueued on `stream` of `device`; it must outlive them.
-// Registering again for the same (device, stream) replaces the buffer.  The library itself never allocates.
-int sniper_depthwise3x3_set_wgrad_workspace(void* ws, size_t bytes, int device, void* stream) {
-  SN_CHECK(device >= 0, "depthwise3x3_set_wgrad_workspace: device (%d) must be >= 0", device);
-  SN_CHECK(ws != nullptr, "depthwise3x3_set_wgrad_workspace: ws must not be null");
-  SN_CHECK((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "depthwise3x3_set_wgrad_workspace: ws must be 16-byte aligned");
-  SN_CHECK(bytes >= sniper_depthwise3x3_wgrad_workspace_bytes(),
-           "depthwise3x3_set_wgrad_workspace: bytes (%zu) is smaller than sniper_depthwise3x3_wgrad_workspace_bytes() (%zu)",
-           bytes, sniper_depthwise3x3_wgrad_workspace_bytes());
-  const cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < g_wg_ws_n; ++i)
-    if (g_wg_ws[i].device == device && g_wg_ws[i].stream == st) {
-      g_wg_ws[i].ws = ws;
-      return 0;
-    }
-  SN_CHECK(g_wg_ws_n < kWgWsEntries, "depthwise3x3_set_wgrad_workspace: more than %d (device, stream) pairs",
-           kWgWsEntries);
-  g_wg_ws[g_wg_ws_n++] = WgWs{device, st, ws};
-  return 0;
-}
-
 // dw[9,C] += sum over pixels of dy * shifted x (fp32; one addition into the existing value: zero dw for kWriteTo).
 // The block partials go through the workspace registered for (current device, stream) and are added in a fixed
 // order, so every launch gives the same bits.
@@ -298,18 +256,12 @@ int sniper_depthwise3x3_wgrad(const void* x, long ldx, const void* dy, long lddy
   SN_CHECK(reinterpret_cast<uintptr_t>(dy) % vec == 0, "depthwise3x3_wgrad: dy must be %d-byte aligned", (int)vec);
   SN_CHECK(dw != nullptr, "depthwise3x3_wgrad: dw must not be null");
   SN_CHECK((reinterpret_cast<uintptr_t>(dw) & 3) == 0, "depthwise3x3_wgrad: dw must be 4-byte aligned");
-  SN_CHECK(9L * C <= kWgSlabFloats, "depthwise3x3_wgrad: C (%d) exceeds the workspace's %ld channels", C,
-           kWgSlabFloats / 9);
+  SN_CHECK(9L * C <= sn::kWgSlabFloats, "depthwise3x3_wgrad: C (%d) exceeds the workspace's %ld channels", C,
+           sn::kWgSlabFloats / 9);
+  sn::StreamWs ws;
+  if (sn::stream_workspace(stream, &ws, "depthwise3x3_wgrad")) return -1;
+  float* part = ws.slab;
   cudaStream_t st = (cudaStream_t)stream;
-  bool any = false;
-  for (int i = 0; i < g_wg_ws_n; ++i) any |= g_wg_ws[i].stream == st;
-  SN_CHECK(any, "depthwise3x3_wgrad: no workspace registered for this stream (sniper_depthwise3x3_set_wgrad_workspace)");
-  int dev = -1;
-  SN_CUDA(cudaGetDevice(&dev));
-  float* part = nullptr;
-  for (int i = 0; i < g_wg_ws_n; ++i)
-    if (g_wg_ws[i].device == dev && g_wg_ws[i].stream == st) part = static_cast<float*>(g_wg_ws[i].ws);
-  SN_CHECK(part != nullptr, "depthwise3x3_wgrad: no workspace registered for device %d and this stream", dev);
   const int LC = dwc::wgrad_lc(C), PL = kWgTY * (32 / LC);
   const int gy = sn::div_up(C >> 2, LC);
   const dim3 block(32, kWgTY, 1);
@@ -320,7 +272,7 @@ int sniper_depthwise3x3_wgrad(const void* x, long ldx, const void* dy, long lddy
     gx = ((long)sn::kNumSMs * wgrad_blocks_per_sm(dw_wgrad_kernel<T, S, PW>) + gy - 1) / gy;   /* one wave */         \
     const long gx_max = (strips + PL - 1) / PL;                                                                      \
     if (gx > gx_max) gx = gx_max;                                                                                    \
-    if (gx > kWgSlabFloats / (9L * C)) gx = kWgSlabFloats / (9L * C);                                                \
+    if (gx > sn::kWgSlabFloats / (9L * C)) gx = sn::kWgSlabFloats / (9L * C);                                        \
     if (gx < 1) gx = 1;                                                                                              \
     dw_wgrad_kernel<T, S, PW><<<dim3((unsigned)gx, (unsigned)gy, 1), block, 0, st>>>(                                \
         static_cast<const T*>(x), static_cast<const T*>(dy), part, p);                                              \

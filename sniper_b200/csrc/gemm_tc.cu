@@ -17,7 +17,7 @@
 //   mode 2  WGRAD   C[Co,(tap,ci)] += sum_pix dY[pix,Co] * X[n,h+dh,w+dw,ci]   split-K.  bf16: both operands
 //                   MN-major, wgmma reads the tiles directly (transpose bits).  tf32 (wgmma takes K-major tf32 only),
 //                   stride-1 multi-tap layers over rows of Wo % 32 == 0 pixels: a copy kernel first writes dY^T and X^T
-//                   channel-major into the stream's scratch and the TMA loads those K-major (see WgradFeed); other
+//                   channel-major into the stream's workspace and the TMA loads those K-major (see WgradFeed); other
 //                   layers (wg_xpose): the consumers transpose each MN-major ring stage into a second, K-major ring
 //                   while the wgmma of the previous stage run
 //
@@ -777,42 +777,6 @@ size_t smem_bytes(int stages, int block_n, int xpose) {
   return (size_t)(stages + (xpose ? kXStages : 0)) * (kStageABytes + block_n * 128) + kSmemFixed;
 }
 
-// Split-K workspaces: kTailSlots buffers per device (one per stream using the kernel concurrently) carved out of
-// ONE caller-provided allocation (sniper_gemm_set_tail_workspace; the library itself never allocates).  One buffer
-// holds the parked partial tiles of at most kNumSMs splits (128 x 256 fp32 each) + kNumSMs x 8 arrival counters.
-// Without a registered workspace weight gradients run unsplit.
-constexpr int kTailSlots = 4;
-constexpr int kMaxDevices = 64;
-constexpr size_t kTailWsBytes = (size_t)sn::kNumSMs * 128 * 256 * 4;
-constexpr size_t kTailCntBytes = ((size_t)sn::kNumSMs * 8 * sizeof(int) + 255) / 256 * 256;
-struct TailSlot {
-  cudaStream_t stream;
-  bool used;
-  float4* ws;
-  int* cnt;
-};
-struct TailDevice {
-  bool ready;
-  TailSlot slot[kTailSlots];
-};
-TailDevice g_tail[kMaxDevices];   // host-side table; the entry points are not re-entrant across host threads
-                                  // (documented in include/sniper_b200.h): one host thread drives a device's launches
-
-TailSlot* tail_slot(cudaStream_t stream) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices || !g_tail[dev].ready) return nullptr;
-  TailSlot* sl = g_tail[dev].slot;
-  for (int i = 0; i < kTailSlots; ++i)
-    if (sl[i].used && sl[i].stream == stream) return &sl[i];
-  for (int i = 0; i < kTailSlots; ++i)
-    if (!sl[i].used) {
-      sl[i].used = true;
-      sl[i].stream = stream;
-      return &sl[i];
-    }
-  return nullptr;   // more concurrent streams than slots: run without the tail split
-}
-
 // Decide the tail split of a K-major launch (see GemmParams::tail_*).  SNIPER_GEMM_TAIL=0 disables it.  Only for
 // widths that are a multiple of 32 columns (every layer of the training step; ragged widths keep whole tiles).
 // (A K-slice split of the tail is not offered: its parked partials made graph-replayed steps differ run to run in
@@ -920,7 +884,7 @@ void fill_kmajor(GemmParams& p, int dtype, int block_n) {
 
 // tf32 weight gradient operand feed.  wgmma reads tf32 K-major only and both operands are pixel-major.  For stride-1
 // layers with several taps whose output rows are Wo % 32 == 0 pixels (the 3 x 3 layers of the ResNet-101 step), a copy
-// kernel first writes them channel-major into the stream's scratch:
+// kernel first writes them channel-major into the copy area of the stream's workspace:
 //   dY^T [Cout, P], P = NB * Ho * Wo output pixels in k-block order;
 //   X^T  [cols * Cin, NB * Hp * Wo]: one row block per distinct column offset dw of the taps, X^T[j * Cin + ci,
 //        (n, hp, ow)] = X[n, hp - padh, ow + dw_j, ci] over the input rows zero-padded to Hp (padh before the first), so
@@ -939,7 +903,7 @@ struct WgradFeed {
   int tapblk[kMaxTaps];       // row block each tap reads
   long x_pixels;              // pixels per X^T row
   long p_pitch, x_pitch;      // elements per row of dY^T / X^T
-  size_t xt_off, bytes;       // X^T offset in the scratch (256-byte aligned), total bytes
+  size_t xt_off, bytes;       // X^T offset in the copy area (256-byte aligned), total bytes
 };
 
 bool wgrad_copies(int dtype, int ntaps, int stride, int Wo) {
@@ -969,17 +933,6 @@ WgradFeed wgrad_feed(int NB, int H, int Cin, int Cout, int ntaps, const int* tap
   f.bytes = f.xt_off + (size_t)f.blocks * Cin * f.x_pitch * 4;
   return f;
 }
-
-// caller-owned scratch per (device, stream) (sniper_conv2d_wgrad_set_scratch); the library never allocates
-struct WgScratch {
-  int device;
-  cudaStream_t stream;
-  void* ptr;
-  size_t bytes;
-};
-constexpr int kWgScratchEntries = 32;
-WgScratch g_wg_scratch[kWgScratchEntries];
-int g_wg_scratch_n = 0;
 
 struct Epilogue {
   const float* scale;
@@ -1156,20 +1109,20 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
     if (s > total_kb / 8) s = total_kb / 8;
     splits = s < 1 ? 1 : (int)s;
   }
-  // splits are summed deterministically through the stream's tail workspace (one 128 x 256 partial per split and
-  // tile, at most kNumSMs of them); without a registered workspace the weight gradient runs unsplit
+  // splits are summed deterministically through the stream's workspace (one 128 x 256 partial per split and tile, at
+  // most kNumSMs of them)
   const long wg_tiles = (long)(Cout / 128 + (Cout % 128 ? 1 : 0)) * ntaps * p.wg_cin_blocks;
-  TailSlot* slot = splits > 1 ? tail_slot((cudaStream_t)stream) : nullptr;
-  if (!slot) splits = 1;
   while (splits > 1 && (total_kb % splits != 0 || wg_tiles * splits > sn::kNumSMs)) --splits;
-  if (splits > 1) {
-    p.split_park = 1;
-    p.tail_ws = slot->ws;
-    p.tail_cnt = slot->cnt;
-  }
   p.num_kb = (int)(total_kb / splits);
   p.C = dW; p.ldc = (long)ntaps * Cin; p.atomic = 1;
   SN_CHECK(dy_ld >= Cout && x_ld >= Cin && (dy_ld * esz) % 16 == 0 && (x_ld * esz) % 16 == 0, "wgrad: bad ld");
+  sn::StreamWs ws = {};
+  if ((splits > 1 || copies) && sn::stream_workspace(stream, &ws, "wgrad")) return -1;
+  if (splits > 1) {
+    p.split_park = 1;
+    p.tail_ws = ws.partials;
+    p.tail_cnt = ws.counters;
+  }
   const uint32_t ones[4] = {1, 1, 1, 1};
   CUtensorMap ma, mb;
   dim3 grid(Cout / 128 + (Cout % 128 ? 1 : 0), ntaps * p.wg_cin_blocks, splits);
@@ -1190,23 +1143,15 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
     return launch(ma, mb, p, grid, (cudaStream_t)stream);
   }
 
-  // channel-major copies of both operands into the stream's scratch, then the K-major mainloop
+  // channel-major copies of both operands into the copy area of the stream's workspace, then the K-major mainloop
   SN_CHECK((reinterpret_cast<uintptr_t>(dY) & 15) == 0 && (reinterpret_cast<uintptr_t>(X) & 15) == 0,
            "wgrad: dY and X must be 16-byte aligned");
   const WgradFeed f = wgrad_feed(NB, H, Cin, Cout, ntaps, tap_dh, tap_dw, Ho, Wo);
-  int dev = -1;
-  SN_CUDA(cudaGetDevice(&dev));
-  const WgScratch* sc = nullptr;
-  for (int i = 0; i < g_wg_scratch_n; ++i)
-    if (g_wg_scratch[i].device == dev && g_wg_scratch[i].stream == (cudaStream_t)stream) sc = &g_wg_scratch[i];
-  SN_CHECK(sc != nullptr,
-           "wgrad: no tf32 operand scratch registered for device %d and this stream (sniper_conv2d_wgrad_set_scratch)",
-           dev);
-  SN_CHECK(sc->bytes >= f.bytes,
-           "wgrad: the stream's tf32 operand scratch holds %zu bytes, this call needs %zu (sniper_conv2d_wgrad_scratch_bytes)",
-           sc->bytes, f.bytes);
-  float* dyt = static_cast<float*>(sc->ptr);
-  float* xt = reinterpret_cast<float*>(static_cast<uint8_t*>(sc->ptr) + f.xt_off);
+  SN_CHECK(ws.copy_bytes >= f.bytes,
+           "wgrad: the stream's workspace has a %zu-byte copy area, this call needs %zu (sniper_set_stream_workspace, "
+           "sniper_conv2d_wgrad_scratch_bytes)", ws.copy_bytes, f.bytes);
+  float* dyt = static_cast<float*>(ws.copies);
+  float* xt = reinterpret_cast<float*>(static_cast<uint8_t*>(ws.copies) + f.xt_off);
   {
     const uint64_t pb = (uint64_t)f.p_pitch * 4;
     const uint64_t d[4] = {(uint64_t)pixels, (uint64_t)Cout, 1, 1};
@@ -1240,57 +1185,13 @@ int sniper_conv2d_wgrad_nhwc(const void* dY, long dy_ld, const void* X, long x_l
   return launch(ma, mb, p, grid, (cudaStream_t)stream);
 }
 
-// Bytes of the tf32 operand scratch sniper_conv2d_wgrad_nhwc needs for a geometry (host only; 0 where the kernel reads
-// the operands in place: bf16, and tf32 layers without copies, see WgradFeed).  Same arguments as that entry point.
+// Bytes of the tf32 operand copy area sniper_conv2d_wgrad_nhwc needs in the stream's workspace for a geometry (host
+// only; 0 where the kernel reads the operands in place: bf16, and tf32 layers without copies, see WgradFeed).  Same
+// arguments as that entry point.
 size_t sniper_conv2d_wgrad_scratch_bytes(int NB, int H, int W, int Cin, int Cout, int ntaps, const int* tap_dh,
                                          const int* tap_dw, int stride, int Ho, int Wo, int dtype) {
   if (!wgrad_copies(dtype, ntaps, stride, Wo) || ntaps > kMaxTaps || !tap_dh || !tap_dw) return 0;
   return wgrad_feed(NB, H, Cin, Cout, ntaps, tap_dh, tap_dw, Ho, Wo).bytes;
-}
-
-// Registers a caller-owned device buffer (256-byte aligned, no initialisation) as the tf32 operand scratch of the
-// weight gradients enqueued on `stream` of `device`; it must outlive them.  Registering again for the same (device,
-// stream) replaces the buffer.  The library itself never allocates.
-int sniper_conv2d_wgrad_set_scratch(void* ptr, size_t bytes, int device, void* stream) {
-  SN_CHECK(device >= 0, "conv2d_wgrad_set_scratch: device (%d) must be >= 0", device);
-  SN_CHECK(ptr != nullptr, "conv2d_wgrad_set_scratch: ptr must not be null");
-  SN_CHECK((reinterpret_cast<uintptr_t>(ptr) & 255) == 0, "conv2d_wgrad_set_scratch: ptr must be 256-byte aligned");
-  const cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < g_wg_scratch_n; ++i)
-    if (g_wg_scratch[i].device == device && g_wg_scratch[i].stream == st) {
-      g_wg_scratch[i].ptr = ptr;
-      g_wg_scratch[i].bytes = bytes;
-      return 0;
-    }
-  SN_CHECK(g_wg_scratch_n < kWgScratchEntries, "conv2d_wgrad_set_scratch: more than %d (device, stream) pairs",
-           kWgScratchEntries);
-  g_wg_scratch[g_wg_scratch_n++] = WgScratch{device, st, ptr, bytes};
-  return 0;
-}
-
-// Bytes sniper_gemm_set_tail_workspace expects (per device).
-size_t sniper_gemm_tail_workspace_bytes(void) { return (size_t)kTailSlots * (kTailWsBytes + kTailCntBytes); }
-
-// Registers a caller-owned, ZERO-FILLED device buffer of sniper_gemm_tail_workspace_bytes() bytes for `device`; it must
-// outlive every later launch on that device.  Enables the split-K weight gradient (GemmParams::split_park).
-// ws = NULL unregisters.
-int sniper_gemm_set_tail_workspace(void* ws, size_t bytes, int device) {
-  SN_CHECK(device >= 0 && device < kMaxDevices, "gemm_set_tail_workspace: device %d out of range", device);
-  TailDevice& d = g_tail[device];
-  d.ready = false;
-  if (ws == nullptr) return 0;
-  SN_CHECK(bytes >= sniper_gemm_tail_workspace_bytes(), "gemm_set_tail_workspace: %zu bytes given, %zu needed", bytes,
-           sniper_gemm_tail_workspace_bytes());
-  SN_CHECK((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "gemm_set_tail_workspace: buffer must be 256-byte aligned");
-  uint8_t* p8 = static_cast<uint8_t*>(ws);
-  for (int i = 0; i < kTailSlots; ++i) {
-    d.slot[i].stream = nullptr;
-    d.slot[i].used = false;
-    d.slot[i].ws = reinterpret_cast<float4*>(p8 + (size_t)i * (kTailWsBytes + kTailCntBytes));
-    d.slot[i].cnt = reinterpret_cast<int*>(p8 + (size_t)i * (kTailWsBytes + kTailCntBytes) + kTailWsBytes);
-  }
-  d.ready = true;
-  return 0;
 }
 
 // Host-only query of the launch plan sniper_gemm_nt would use for C[M,N] = A[M,K] * B[N,K]^T with 16-byte aligned,

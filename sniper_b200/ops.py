@@ -233,21 +233,6 @@ def _dt(t):
     return TF32 if t.dtype == torch.float32 else BF16
 
 
-_gemm_ws = {}
-
-
-def _ensure_gemm_workspace(device):
-    """The wgmma kernel's split-K scratch is caller-owned (the library never allocates): one zero-filled torch
-    buffer per device, registered once and kept alive for the life of the process."""
-    idx = device.index if device.index is not None else torch.cuda.current_device()
-    if idx not in _gemm_ws:
-        L = lib()
-        n = L.sniper_gemm_tail_workspace_bytes()
-        buf = torch.zeros(n, dtype=torch.uint8, device=torch.device("cuda", idx))
-        check(L.sniper_gemm_set_tail_workspace(buf.data_ptr(), n, idx))
-        _gemm_ws[idx] = buf
-
-
 def gemm_nt(a, b, *, out=None, scale=None, bias=None, residual=None, relu=False, accumulate=False, out_dtype=None,
             stats=None):
     """C[M,N] = epi(A[M,K] @ B[N,K]^T) on wgmma tensor cores (fp32 storage -> TF32 math, or bf16 operands with fp32
@@ -256,7 +241,6 @@ def gemm_nt(a, b, *, out=None, scale=None, bias=None, residual=None, relu=False,
     assert a.stride(1) == 1 and b.stride(1) == 1
     M, K = a.shape
     N = b.shape[0]
-    _ensure_gemm_workspace(a.device)
     if out is None:
         out = torch.empty(M, N, device=a.device, dtype=out_dtype or a.dtype)
     out_bf16 = out.dtype == torch.bfloat16
@@ -293,7 +277,6 @@ def conv2d_nhwc(x, w, *, kh, kw, stride=1, dil=1, pad=0, out=None, scale=None, b
         Wo = (W + 2 * pad - dil * (kw - 1) - 1) // stride + 1
     else:
         Ho, Wo = out_hw
-    _ensure_gemm_workspace(x.device)
     if out is None:
         out = torch.empty(NB, Ho, Wo, Cout, device=x.device, dtype=out_dtype or x.dtype)
     assert x.dtype == w.dtype and (residual is None or residual.dtype == out.dtype), "bf16 output takes a bf16 residual"
@@ -317,27 +300,30 @@ def _pixel_ld(t):
     return ld
 
 
-_wg_scratch = {}
-_wg_scratch_replaced = []
+_workspaces = {}
+_replaced_workspaces = []
 
 
-def _ensure_wgrad_scratch(nbytes):
-    """The tf32 weight gradient copies its operands channel-major into a caller-owned scratch (the library never
-    allocates): one buffer per (device, stream), because launches on different streams may overlap, grown to the next
-    power of two when a call needs more.  A replaced buffer is kept alive for the life of the process, because a
-    captured CUDA graph may still hold its address."""
-    if nbytes == 0:
-        return
+def _stream_workspace(copy_bytes=0):
+    """The device scratch of the weight gradients on the current stream (the library never allocates): one buffer per
+    (device, stream), because launches on different streams may overlap.  It holds the split-K partials and counters
+    and the depthwise slab (the fixed part), then at least `copy_bytes` for the tf32 operand copies; it is grown to
+    the fixed part + the next power of two when a call needs more.  Only the fixed part is zeroed, on the current
+    stream (a memset node when captured), because the split-K counters must start at zero.  A replaced buffer is kept
+    alive for the life of the process, because a captured CUDA graph may still hold its address."""
     idx, st = torch.cuda.current_device(), _stream()
-    cur = _wg_scratch.get((idx, st))
-    if cur is not None and cur.numel() >= nbytes:
-        return
-    n = 1 << (nbytes - 1).bit_length()
+    fixed = lib().sniper_stream_workspace_bytes()
+    cur = _workspaces.get((idx, st))
+    if cur is not None and cur.numel() - fixed >= copy_bytes:
+        return cur
+    n = fixed + (1 << (copy_bytes - 1).bit_length() if copy_bytes else 0)
     buf = torch.empty(n, dtype=torch.uint8, device=torch.device("cuda", idx))
-    check(lib().sniper_conv2d_wgrad_set_scratch(buf.data_ptr(), n, idx, st))
+    buf[:fixed].zero_()
+    check(lib().sniper_set_stream_workspace(buf.data_ptr(), n, idx, st))
     if cur is not None:
-        _wg_scratch_replaced.append(cur)
-    _wg_scratch[(idx, st)] = buf
+        _replaced_workspaces.append(cur)
+    _workspaces[(idx, st)] = buf
+    return buf
 
 
 def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, splits=8, taps=None):
@@ -346,7 +332,6 @@ def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, spl
     _, Ho, Wo, Cout = dy.shape
     dh, dw = taps if taps is not None else conv_taps(kh, kw, dil, pad)
     ntaps = len(dh)
-    _ensure_gemm_workspace(x.device)
     assert dy.dtype == x.dtype and dy.shape[0] == NB
     dy_ld, x_ld = _pixel_ld(dy), _pixel_ld(x)
     if dw_out is None:
@@ -355,8 +340,8 @@ def conv2d_wgrad_nhwc(dy, x, *, kh, kw, stride=1, dil=1, pad=0, dw_out=None, spl
         "dw_out must be a contiguous fp32 [Cout, taps * Cin]"
     _, dhp = _iarr(dh)
     _, dwp = _iarr(dw)
-    _ensure_wgrad_scratch(lib().sniper_conv2d_wgrad_scratch_bytes(NB, H, W, Cin, Cout, ntaps, dhp, dwp, stride, Ho, Wo,
-                                                                   _dt(x)))
+    _stream_workspace(lib().sniper_conv2d_wgrad_scratch_bytes(NB, H, W, Cin, Cout, ntaps, dhp, dwp, stride, Ho, Wo,
+                                                               _dt(x)))
     check(lib().sniper_conv2d_wgrad_nhwc(_ptr(dy), dy_ld, _ptr(x), x_ld, NB, H, W, Cin, Cout, ntaps, dhp,
                                          dwp, stride, Ho, Wo,
                                          _ptr(dw_out), _dt(x), splits, _stream()))
@@ -972,30 +957,13 @@ def depthwise3x3_dgrad(dy, w, in_hw, stride=1, out=None):
     return out
 
 
-_dw_ws = {}
-
-
-def _ensure_dw_wgrad_workspace():
-    """The depthwise weight gradient sums its block partials in a caller-owned slab (the library never allocates): one
-    buffer per (device, stream), because launches on different streams (WgradScheduler's side stream, the main
-    stream) may overlap.  Registered once and kept alive for the life of the process, so that captured CUDA graphs
-    keep a valid address."""
-    idx, st = torch.cuda.current_device(), _stream()
-    if (idx, st) not in _dw_ws:
-        L = lib()
-        n = L.sniper_depthwise3x3_wgrad_workspace_bytes()
-        buf = torch.empty(n, dtype=torch.uint8, device=torch.device("cuda", idx))
-        check(L.sniper_depthwise3x3_set_wgrad_workspace(buf.data_ptr(), n, idx, st))
-        _dw_ws[(idx, st)] = buf
-
-
 def depthwise3x3_wgrad(x, dy, dw, stride=1):
     """dw[9,C] (fp32) += correlation of dy with the shifted input, summed in a fixed order (two calls give the same
     bits)."""
     NB, H, W, C = x.shape
     assert dw.shape == (9, C) and dw.dtype == torch.float32 and dw.is_contiguous() and x.dtype == dy.dtype
     assert x.is_contiguous() and dy.is_contiguous()
-    _ensure_dw_wgrad_workspace()
+    _stream_workspace()
     check(lib().sniper_depthwise3x3_wgrad(_ptr(x), x.stride(2), _ptr(dy), dy.stride(2), _ptr(dw), NB, H, W, C, stride,
                                           _sdt(x), _stream()))
     return dw

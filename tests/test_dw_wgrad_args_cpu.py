@@ -1,9 +1,10 @@
-"""Argument validation of the depthwise weight gradient and its workspace (csrc/depthwise.cu).
+"""Argument validation of the depthwise weight gradient (csrc/depthwise.cu) and of the stream workspace registration
+it shares with the wgmma weight gradient (csrc/capi_common.cu).
 
-sniper_depthwise3x3_wgrad reads x and dy as 4-channel vectors, adds into dw, and sums its block partials in a
-caller-owned workspace registered per (device, stream) with sniper_depthwise3x3_set_wgrad_workspace.  A bad shape, a
-null or misaligned pointer, or a missing, null, misaligned or too small workspace must be refused BEFORE any CUDA
-call, with a message naming the argument.  Every call below is built from fabricated, never dereferenced addresses and
+sniper_depthwise3x3_wgrad reads x and dy as 4-channel vectors, adds into dw, and sums its block partials in the slab of
+the caller-owned workspace registered per (device, stream) with sniper_set_stream_workspace.  A bad shape, a null or
+misaligned pointer, or a missing, null, misaligned or too small workspace must be refused BEFORE any CUDA call, with a
+message naming the argument.  Every call below is built from fabricated, never dereferenced addresses and
 violates exactly one rule.  On a machine without a device a check that wrongly passed would reach cudaGetDevice and
 fail with a CUDA error instead of the expected message, so the message match also proves that no CUDA call was made.
 There is deliberately no GPU variant of these tests."""
@@ -24,7 +25,7 @@ WS = "ws bytes device stream"
 
 
 def _ws_bytes():
-    return _lib.lib().sniper_depthwise3x3_wgrad_workspace_bytes()
+    return _lib.lib().sniper_stream_workspace_bytes()
 
 
 def _call(name, order, args):
@@ -40,7 +41,7 @@ def _ws_good():
 @pytest.fixture(scope="module", autouse=True)
 def registered():
     """ST gets a (fabricated) workspace, so that the shape checks are reached with a workspace in place."""
-    rc, msg = _call("sniper_depthwise3x3_set_wgrad_workspace", WS, _ws_good())
+    rc, msg = _call("sniper_set_stream_workspace", WS, _ws_good())
     assert rc == 0, msg
 
 
@@ -57,44 +58,47 @@ def _bad_ws(pattern, **change):
     a = _ws_good()
     assert all(k in a for k in change)
     a.update(change)
-    rc, msg = _call("sniper_depthwise3x3_set_wgrad_workspace", WS, a)
+    rc, msg = _call("sniper_set_stream_workspace", WS, a)
     assert rc == -1
     assert re.search(pattern, msg), msg
 
 
 def test_workspace_size_covers_a_full_wave_of_the_widest_blocks():
-    # 132 SMs x 4 blocks x 9 taps x 128 channels of fp32 partials; the same for every shape
-    assert _ws_bytes() == 132 * 4 * 9 * 128 * 4
+    # the fixed part, each region 256-byte aligned: split-K parked partials (132 tiles of 128 x 256 fp32), arrival
+    # counters (132 x 8 ints), then the slab: 132 SMs x 4 blocks x 9 taps x 128 channels of fp32 partials
+    assert _ws_bytes() == 132 * 128 * 256 * 4 + 4352 + 132 * 4 * 9 * 128 * 4
 
 
 def test_registration_accepts_a_well_formed_workspace():
-    rc, msg = _call("sniper_depthwise3x3_set_wgrad_workspace", WS, dict(_ws_good(), bytes=_ws_bytes() + 4096))
+    rc, msg = _call("sniper_set_stream_workspace", WS, dict(_ws_good(), bytes=_ws_bytes() + 4096))
     assert rc == 0, msg
-    rc, msg = _call("sniper_depthwise3x3_set_wgrad_workspace", WS, _ws_good())      # again: replaces the buffer
+    rc, msg = _call("sniper_set_stream_workspace", WS, _ws_good())      # again: replaces the buffer
     assert rc == 0, msg
 
 
 def test_null_workspace():
-    _bad_ws(r"depthwise3x3_set_wgrad_workspace: ws must not be null", ws=0)
+    _bad_ws(r"set_stream_workspace: ws must not be null", ws=0)
 
 
-@pytest.mark.parametrize("off", [4, 8, 12])
+@pytest.mark.parametrize("off", [4, 8, 12, 16, 64, 128])
 def test_misaligned_workspace(off):
-    _bad_ws(r"depthwise3x3_set_wgrad_workspace: ws must be 16-byte aligned", ws=V[2] + off)
+    _bad_ws(r"set_stream_workspace: ws must be 256-byte aligned", ws=V[2] + off)
 
 
 def test_too_small_workspace():
     n = _ws_bytes()
-    _bad_ws(r"depthwise3x3_set_wgrad_workspace: bytes \(%d\) is smaller than .* \(%d\)" % (n - 4, n), bytes=n - 4)
-    _bad_ws(r"depthwise3x3_set_wgrad_workspace: bytes \(0\) is smaller", bytes=0)
+    _bad_ws(r"set_stream_workspace: bytes \(%d\) is smaller than sniper_stream_workspace_bytes\(\) \(%d\)" % (n - 4, n),
+            bytes=n - 4)
+    _bad_ws(r"set_stream_workspace: bytes \(0\) is smaller", bytes=0)
 
 
 def test_negative_device():
-    _bad_ws(r"depthwise3x3_set_wgrad_workspace: device \(-1\) must be >= 0", device=-1)
+    _bad_ws(r"set_stream_workspace: device \(-1\) must be >= 0", device=-1)
 
 
 def test_no_workspace_for_the_stream():
-    _bad_wg(r"depthwise3x3_wgrad: no workspace registered for this stream", stream=ST_NONE)
+    _bad_wg(r"depthwise3x3_wgrad: no workspace registered for this stream \(sniper_set_stream_workspace\)",
+            stream=ST_NONE)
 
 
 @pytest.mark.parametrize("dtype", [-1, 2])

@@ -391,7 +391,7 @@ def test_bias_gradient_colsum_exact():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# split-K workspace slots: per stream, and under graph replay
+# split-K through the stream's workspace: on any number of streams, at once, and under graph replay
 # ---------------------------------------------------------------------------------------------------------------------
 def _split_k_problem(dt, seed):
     """1 x 1 weight gradient over 4 x 32 x 32 pixels, Cin 256: 128 / 64 k-blocks, tiles 1 / 2, 8 splits either way"""
@@ -400,47 +400,36 @@ def _split_k_problem(dt, seed):
     return dy, x, _wgrad_ref(dy, x, 1, 1, 1, 0)
 
 
-# The registered split-K workspace: kTailSlots = 4 slots of [parked partials: 132 x 128 x 256 fp32 | arrival counters].
-# A stream claims the first free slot at its first split launch and keeps it; a stream that finds none runs unsplit.
-TAIL_SLOTS, PARKED_BYTES = 4, 132 * 128 * 256 * 4
+# The stream's workspace (ops._stream_workspace) starts with the split-K regions: [parked partials: 132 x 128 x 256 fp32 |
+# arrival counters: 132 x 8 int32].
+PARKED_BYTES, COUNTER_BYTES = 132 * 128 * 256 * 4, 132 * 8 * 4
 POISON = -12345.0       # no parked partial of _split_k_problem can take this value (|partial| <= 4096 pixels)
 
 
-def _slot_views(ws):
-    per = ws.numel() // TAIL_SLOTS
-    return [(ws[s * per:s * per + PARKED_BYTES].view(torch.float32), ws[s * per + PARKED_BYTES:(s + 1) * per])
-            for s in range(TAIL_SLOTS)]
-
-
-def _reset_split_k_slots():
-    """Zero the registered workspace and register it again: every slot free and every counter zero, whichever streams
-    claimed slots earlier in this process."""
+def _split_k_views(stream):
+    """(parked partials, arrival counters) of the stream's workspace"""
     from sniper_b200 import ops
-    from sniper_b200._lib import check, lib
-    ops._ensure_gemm_workspace(torch.device("cuda"))
-    ws = ops._gemm_ws[torch.cuda.current_device()]
-    torch.cuda.synchronize()
-    ws.zero_()
-    torch.cuda.synchronize()
-    check(lib().sniper_gemm_set_tail_workspace(ws.data_ptr(), ws.numel(), torch.cuda.current_device()))
-    return ws
+    with torch.cuda.stream(stream):
+        ws = ops._stream_workspace()
+    return ws[:PARKED_BYTES].view(torch.float32), ws[PARKED_BYTES:PARKED_BYTES + COUNTER_BYTES].view(torch.int32)
 
 
-def _poison(ws):
-    for parked, _ in _slot_views(ws):
-        parked.fill_(POISON)
+def _poison(streams):
+    torch.cuda.synchronize()
+    for s in streams:
+        parked, _ = _split_k_views(s)
+        with torch.cuda.stream(s):          # after the zero fill of a workspace created just now
+            parked.fill_(POISON)
     torch.cuda.synchronize()
 
 
-def _slots_written(ws):
-    """Slots whose parked-partials region a launch wrote since the last _poison (i.e. that ran a split-K reduction)"""
+def _split_k_ran(stream):
+    """whether a launch on the stream wrote its parked-partials region since the last _poison (i.e. ran a split-K
+    reduction), with every arrival counter back at zero"""
     torch.cuda.synchronize()
-    return [s for s, (parked, _) in enumerate(_slot_views(ws)) if bool((parked != POISON).any())]
-
-
-def _assert_counters_clean(ws):
-    for s, (_, cnt) in enumerate(_slot_views(ws)):
-        assert not bool(cnt.any()), "split-K counters of slot %d were left non-zero" % s
+    parked, cnt = _split_k_views(stream)
+    assert not bool(cnt.any()), "split-K counters were left non-zero"
+    return bool((parked != POISON).any())
 
 
 def _split_k_on_streams(dt, streams, seed):
@@ -464,29 +453,64 @@ def _split_k_on_streams(dt, streams, seed):
 
 
 @pytest.mark.parametrize("dt", DTS)
-def test_split_k_slots_are_per_stream(dt):
-    """Split-K weight gradients on two streams at once take two different slots and are each exact.  Five more streams
-    then find the 2 remaining slots: the first two take them, the other three run unsplit, and all five stay exact.
-    The workspace is registered afresh first, so the slot count does not depend on earlier tests."""
-    ws = _reset_split_k_slots()
+def test_split_k_on_concurrent_streams(dt):
+    """Split-K weight gradients on seven streams at once each run split in their own stream's workspace and are each
+    exact."""
     streams = [torch.cuda.Stream() for _ in range(7)]
     assert len({s.cuda_stream for s in streams} | {torch.cuda.current_stream().cuda_stream}) == 8
-    _poison(ws)
-    _split_k_on_streams(dt, streams[:2], 100)
-    assert _slots_written(ws) == [0, 1], "the two streams did not run split-K in their own slots"
-    _poison(ws)
-    _split_k_on_streams(dt, streams[2:], 200)
-    # slots 0 and 1 stay with the first two streams: only 2 of the 5 new streams ran split, 3 ran unsplit
-    assert _slots_written(ws) == [2, 3], "expected exactly the two free slots to be used by the five streams"
-    _assert_counters_clean(ws)
+    _poison(streams)
+    _split_k_on_streams(dt, streams, 100)
+    assert [_split_k_ran(s) for s in streams] == [True] * 7, "not every stream ran split-K"
+
+
+def test_split_k_is_byte_equal_on_every_stream():
+    """The split count depends on the shape alone: the same 8-split weight gradient on random fp32 operands gives the
+    same bytes on six fresh streams, and each of them runs the split-K reduction, however many streams this process
+    has used before."""
+    from sniper_b200 import ops
+    g = _gen(400)
+    dy = torch.randn(4, 32, 32, 96, device="cuda", generator=g)
+    x = torch.randn(4, 32, 32, 256, device="cuda", generator=g)
+    streams = [torch.cuda.Stream() for _ in range(6)]
+    assert len({s.cuda_stream for s in streams}) == 6
+    _poison(streams)
+    outs = []
+    for s in streams:
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            outs.append(ops.conv2d_wgrad_nhwc(dy, x, kh=1, kw=1, splits=8))
+    torch.cuda.synchronize()
+    for i, dw in enumerate(outs):
+        assert torch.equal(dw.view(torch.int32), outs[0].view(torch.int32)), "stream %d differs from stream 0" % i
+    assert [_split_k_ran(s) for s in streams] == [True] * 6, "not every stream ran split-K"
+
+
+@pytest.mark.parametrize("dt", DTS)
+def test_split_k_on_an_unregistered_stream_is_refused(dt):
+    """A split-K launch needs its stream's workspace: on a fabricated stream handle nothing was registered for, the
+    call is refused before any launch and dW stays untouched."""
+    import ctypes
+    from sniper_b200._lib import lib
+    dy, x, ref = _split_k_problem(dt, 500)
+    dw = torch.zeros(ref.shape, device="cuda")
+    NB, H, W, Cin = x.shape
+    Cout = dy.shape[3]
+    zero = ctypes.c_int(0)
+    L = lib()
+    rc = L.sniper_conv2d_wgrad_nhwc(dy.data_ptr(), Cout, x.data_ptr(), Cin, NB, H, W, Cin, Cout, 1,
+                                    ctypes.addressof(zero), ctypes.addressof(zero), 1, H, W, dw.data_ptr(),
+                                    0 if dt == "tf32" else 1, 8, 0x7f00beef2000)
+    err = L.sniper_last_error().decode()
+    assert rc != 0 and "wgrad: no workspace registered for this stream (sniper_set_stream_workspace)" in err, err
+    torch.cuda.synchronize()
+    assert not bool(dw.any())
 
 
 def test_graph_replay_column_pieces_and_split_k():
-    """One CUDA graph holding a column-piece GEMM and a split-K weight gradient, captured on a stream that holds a slot
-    and replayed twice: each replay runs the split-K reduction (it writes the slot's parked partials), equals the exact
+    """One CUDA graph holding a column-piece GEMM and a split-K weight gradient, captured on a stream and replayed
+    twice: each replay runs the split-K reduction (it writes the capture stream's parked partials), equals the exact
     results, and leaves every arrival counter at zero."""
     from sniper_b200 import ops
-    ws = _reset_split_k_slots()
     g = _gen(300)
     M, N, K = 20480, 256, 4 * 32            # 160 tiles, last wave 28 -> 64-column pieces
     a, b = _operands(g, "tf32", (M, K), (N, K))
@@ -495,15 +519,15 @@ def test_graph_replay_column_pieces_and_split_k():
     c = torch.zeros(M, N, device="cuda")
     dw = torch.zeros(ref_w.shape, device="cuda")
     cs = torch.cuda.Stream()
-    _poison(ws)
+    _poison([cs])
     cs.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(cs):             # eager on the capture stream first: it claims slot 0
+    with torch.cuda.stream(cs):             # eager on the capture stream first
         ops.gemm_nt(a, b, out=c)
         ops.conv2d_wgrad_nhwc(dy, x, kh=1, kw=1, dw_out=dw, splits=8)
     torch.cuda.synchronize()
     _same(c, ref_c, torch.float32, "eager gemm")
     _same(dw, ref_w, torch.float32, "eager wgrad")
-    assert _slots_written(ws) == [0]
+    assert _split_k_ran(cs)
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph, stream=cs):
         dw.zero_()
@@ -512,13 +536,12 @@ def test_graph_replay_column_pieces_and_split_k():
     for i in range(2):
         c.fill_(-5.0)
         dw.fill_(-5.0)
-        _poison(ws)
+        _poison([cs])
         graph.replay()
         torch.cuda.synchronize()
         _same(c, ref_c, torch.float32, "replay %d gemm" % i)
         _same(dw, ref_w, torch.float32, "replay %d wgrad" % i)
-        assert _slots_written(ws) == [0], "replay %d did not run the split-K reduction" % i
-        _assert_counters_clean(ws)
+        assert _split_k_ran(cs), "replay %d did not run the split-K reduction" % i
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -32,7 +32,7 @@ def test_abi_header_matches_library_and_bindings():
         assert codes == _lib.SIGNATURES[name][1], "%s: header %s vs ctypes %s" % (name, codes, _lib.SIGNATURES[name][1])
     for name in _lib.SIGNATURES:
         assert any(n == name for n, _ in protos), name + " missing from the header"
-    assert L.sniper_abi_version() == 2
+    assert L.sniper_abi_version() == 3
 
 
 def _config1_boxes(seed, n, W=1333, H=800):

@@ -1,11 +1,11 @@
 """The tf32 weight gradient's channel-major operand copies (csrc/gemm_tc.cu, WgradFeed) on the device.
 
 For stride-1 layers with several taps over rows of Wo % 32 == 0 pixels, sniper_conv2d_wgrad_nhwc copies dY and X
-channel-major into a scratch registered per (device, stream) and runs the K-major wgmma mainloop on the copies; other
-tf32 layers transpose in the kernel.  What the exact table of test_gemm_exact_gpu.py cannot see:
-  * the scratch grows on a stream, and a graph captured on another stream (whose scratch is allocated during the
+channel-major into the copy area of the workspace registered per (device, stream) and runs the K-major wgmma mainloop
+on the copies; other tf32 layers transpose in the kernel.  What the exact table of test_gemm_exact_gpu.py cannot see:
+  * the copy area grows on a stream, and a graph captured on another stream (whose workspace is allocated during the
     capture) replays to the same bytes as eager calls;
-  * a tf32 call on a stream without a scratch, or with too small a one, is refused before any launch;
+  * a tf32 call on a stream without a workspace, or with too small a copy area, is refused before any launch;
   * the step's own geometries at 2 chips, bit for bit against float64 on integer operands: the 3 x 3 layer over 3072
     channels at 32 x 32 (the RPN conv, from copies), and the transposing path's 3 x 3 stride-2 layer at 128 -> 64 and
     1 x 1 stride-2 shortcut.
@@ -52,19 +52,27 @@ def test_step_geometry_is_integer_exact(NB, H, Cin, Cout, k, stride, dil, pad):
         assert torch.equal(dw.double(), ref), (splits, (dw.double() - ref).abs().max().item())
 
 
+def _fresh_workspace(stream):
+    """torch hands out pool streams round-robin, so `stream` may be a handle an earlier test grew a workspace on: retire
+    that workspace (kept alive like a replaced one), so that the next call on the stream allocates afresh"""
+    key = (torch.cuda.current_device(), stream.cuda_stream)
+    if key in ops._workspaces:
+        ops._replaced_workspaces.append(ops._workspaces.pop(key))
+
+
 def test_scratch_growth_and_graph_replay_on_another_stream():
     gen = torch.Generator().manual_seed(5)
     small_x, small_dy = torch.randn(1, 4, 32, 64, generator=gen).cuda(), torch.randn(1, 4, 32, 64, generator=gen).cuda()
     x, dy = torch.randn(2, 64, 64, 256, generator=gen).cuda(), torch.randn(2, 64, 64, 128, generator=gen).cuda()
     args = dict(kh=3, kw=3, pad=1, splits=4)
     s1 = torch.cuda.Stream()
+    _fresh_workspace(s1)
     s1.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s1):
         ops.conv2d_wgrad_nhwc(small_dy, small_x, **args)
-        key = (torch.cuda.current_device(), s1.cuda_stream)
-        n_small = ops._wg_scratch[key].numel()
-        eager = ops.conv2d_wgrad_nhwc(dy, x, **args)          # needs more: the stream's scratch grows
-        assert ops._wg_scratch[key].numel() > n_small
+        n_small = ops._stream_workspace().numel()
+        eager = ops.conv2d_wgrad_nhwc(dy, x, **args)          # needs more: the stream's workspace grows
+        assert ops._stream_workspace().numel() > n_small
         eager2 = ops.conv2d_wgrad_nhwc(dy, x, **args)
     torch.cuda.current_stream().wait_stream(s1)
     torch.cuda.synchronize()
@@ -74,6 +82,7 @@ def test_scratch_growth_and_graph_replay_on_another_stream():
 
     dw = torch.zeros_like(eager)
     s2 = torch.cuda.Stream()
+    _fresh_workspace(s2)
     g = torch.cuda.CUDAGraph()
     with torch.cuda.graph(g, stream=s2):
         dw.zero_()
@@ -103,11 +112,11 @@ def test_tf32_call_without_scratch_is_refused():
     x, dy = torch.ones(1, 32, 32, 64, device="cuda"), torch.ones(1, 32, 32, 64, device="cuda")
     dw = torch.zeros(64, 9 * 64, device="cuda")
     rc, err = _raw_wgrad(dy, x, dw, 0x7f00beef0000)
-    assert rc != 0 and "no tf32 operand scratch registered" in err, err
-    buf = torch.empty(1 << 16, dtype=torch.uint8, device="cuda")
-    _lib.check(_lib.lib().sniper_conv2d_wgrad_set_scratch(buf.data_ptr(), buf.numel(), torch.cuda.current_device(),
-                                                          0x7f00beef1000))
+    assert rc != 0 and "no workspace registered for this stream (sniper_set_stream_workspace)" in err, err
+    L = _lib.lib()
+    buf = torch.zeros(L.sniper_stream_workspace_bytes() + (1 << 16), dtype=torch.uint8, device="cuda")
+    _lib.check(L.sniper_set_stream_workspace(buf.data_ptr(), buf.numel(), torch.cuda.current_device(), 0x7f00beef1000))
     rc, err = _raw_wgrad(dy, x, dw, 0x7f00beef1000)
-    assert rc != 0 and "this call needs" in err, err
+    assert rc != 0 and "65536-byte copy area, this call needs" in err, err
     torch.cuda.synchronize()
     assert not dw.any().item()

@@ -1,15 +1,14 @@
-"""The tf32 weight gradient's operand scratch (csrc/gemm_tc.cu, WgradFeed), host only.
+"""The tf32 weight gradient's operand copy area (csrc/gemm_tc.cu, WgradFeed), host only.
 
 For stride-1 layers with several taps over rows of Wo % 32 == 0 pixels, sniper_conv2d_wgrad_nhwc copies dY and X
-channel-major into a caller-owned scratch before its K-major mainloop; other layers and bf16 need none.
-sniper_conv2d_wgrad_scratch_bytes must give the size of that layout for a geometry, restated here in Python: dY^T
+channel-major into the copy area of the stream's workspace before its K-major mainloop; other layers and bf16 need
+none.  sniper_conv2d_wgrad_scratch_bytes must give the size of that layout for a geometry, restated here in Python: dY^T
 [Cout, P] with P = NB * Ho * Wo, its row pitch rounded up to 16 bytes, then at the next 256-byte boundary X^T
 [cols * Cin, NB * Hp * Wo], one block of Cin rows per distinct column offset dw of the taps, over the input rows
 zero-padded to Hp.
 """
 import ctypes
 import os
-import re
 import sys
 
 import numpy as np
@@ -107,24 +106,3 @@ def test_ragged_pitch_rounds_to_16_bytes():
     """3 x 3 over 1 x 3 x 32: P = 96; dY^T 33 x 96 floats is rounded up to 256 bytes, X^T 3 x 64 rows of 5 x 32"""
     g = geometry(1, 3, 32, 64, 33, 3, pad=1)
     assert query(*g) == _round(33 * 96 * 4, 256) + 3 * 64 * 160 * 4
-
-
-SET = "ptr bytes device stream"
-
-
-def _set(**kw):
-    args = dict(ptr=0x7f0000100000, bytes=1 << 20, device=0, stream=0x7f00dead0000)
-    args.update(kw)
-    L = _lib.lib()
-    rc = L.sniper_conv2d_wgrad_set_scratch(*[args[k] for k in SET.split()])
-    return rc, L.sniper_last_error().decode()
-
-
-@pytest.mark.parametrize("kw,msg", [
-    (dict(ptr=0), "ptr must not be null"),
-    (dict(ptr=0x7f0000100010), "ptr must be 256-byte aligned"),
-    (dict(device=-1), r"device \(-1\) must be >= 0"),
-])
-def test_set_scratch_refuses_bad_arguments(kw, msg):
-    rc, err = _set(**kw)
-    assert rc != 0 and re.search(msg, err), err

@@ -8,6 +8,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DOC = {
     "sniper_last_error": "Thread-local message of the last failing call.  Mirrors MXGetLastError (SNIPER-mxnet/include/mxnet/c_api.h:196-204).",
     "sniper_abi_version": "ABI version of this library (bumped on any signature change).",
+    "sniper_stream_workspace_bytes": "Size of the fixed part of a stream workspace: the split-K parked partials and arrival counters of sniper_conv2d_wgrad_nhwc and the block-partial slab of sniper_depthwise3x3_wgrad, each 256-byte aligned, in this order; the tf32 operand copy area (sniper_conv2d_wgrad_scratch_bytes) follows it.",
+    "sniper_set_stream_workspace": "Registers a caller-owned device buffer (256-byte aligned, at least sniper_stream_workspace_bytes() bytes, must outlive later launches) as the workspace of the launches on one (device, stream); registering again replaces it. Its counter region must be zero when it is registered; the kernels leave it zero. The library itself never allocates device memory.",
     "sniper_multi_proposal_target_workspace_bytes": "Scratch bytes for sniper_multi_proposal_target_fwd: replaces ResourceRequest::kTempSpace of MultiProposalTargetProp (multi_proposal_target-inl.h:143-146).",
     "sniper_generate_anchors": "Host helper, utils::GenerateAnchors (multi_proposal_target.cu:75-114): out[nr*ns,4], ratio-major.",
     "sniper_proposal_decode": "K1: utils::getProps (multi_proposal_target.cu:263-331). Anchor shift + bbox_transform_inv + clip + min-size / valid-range filters -> SoA boxes float4[B*A*H*W], score, area. layout 0 = NCHW (reference), 1 = NHWC (channel strides given).",
@@ -21,12 +23,9 @@ DOC = {
     "sniper_psroi_bwd": "PSROIPoolingOp::Backward (contrib/psroi_pooling.cu:146-210); accumulates into data_diff.",
     "sniper_gemm_nt": "C[M,N] = epi(A[M,K] * B[N,K]^T) on wgmma (register accumulators, TMA operands). Replaces FullyConnected -> cuBLAS (nn/fully_connected-inl.h) and linalg_gemm (contrib/deformable_convolution-inl.h:148-160). dtype 0 = fp32 storage / TF32 math, 1 = bf16. epi: *scale[n], +bias[n], +residual[m,n], relu; accumulate = red.global.add (fp32 outputs only; refused with out_bf16).",
     "sniper_gemm_plan": "Host-only: the tile width, ring depth, persistent grid and tail split sniper_gemm_nt would choose for a shape (no GPU needed).",
-    "sniper_gemm_tail_workspace_bytes": "Size of the caller-owned scratch the wgmma kernel's split-K weight gradient uses (per device).",
-    "sniper_gemm_set_tail_workspace": "Registers that scratch (zero-filled, caller-owned, must outlive later launches); the library itself never allocates device memory.",
     "sniper_conv2d_nhwc": "NHWC implicit-GEMM convolution on wgmma; also the stride-1/stride-2 data gradient (flipped / parity-split weights, strided output map). Replaces cudnnConvolutionForward / BackwardData (nn/cudnn/cudnn_convolution-inl.h:144,211-266).",
-    "sniper_conv2d_wgrad_nhwc": "Weight gradient dW[Cout, taps*Cin] += dY^T * im2col(X) on wgmma with split-K: bf16 reads the MN-major operands in place, tf32 first copies them channel-major into the stream's registered scratch (sniper_conv2d_wgrad_set_scratch; refused without one). Replaces cudnnConvolutionBackwardFilter (nn/cudnn/cudnn_convolution-inl.h:211-266).",
-    "sniper_conv2d_wgrad_scratch_bytes": "Host-only: bytes of the tf32 operand scratch sniper_conv2d_wgrad_nhwc needs for a geometry (0 for bf16).",
-    "sniper_conv2d_wgrad_set_scratch": "Registers that scratch (caller-owned, 256-byte aligned, no initialisation, must outlive later launches) for the weight gradients on one (device, stream); registering again replaces it. The library itself never allocates device memory.",
+    "sniper_conv2d_wgrad_nhwc": "Weight gradient dW[Cout, taps*Cin] += dY^T * im2col(X) on wgmma with split-K: bf16 reads the MN-major operands in place, tf32 first copies them channel-major into the copy area of the stream's workspace. Splits > 1 and the copies need the workspace (sniper_set_stream_workspace; refused without one, or with too small a copy area). Replaces cudnnConvolutionBackwardFilter (nn/cudnn/cudnn_convolution-inl.h:211-266).",
+    "sniper_conv2d_wgrad_scratch_bytes": "Host-only: bytes of the tf32 operand copy area sniper_conv2d_wgrad_nhwc needs in the stream's workspace for a geometry (0 for bf16).",
     "sniper_affine_act": "y = act(x*scale[c] + shift[c]) on [M,C] rows (BatchNorm apply + Activation; nn/batch_norm.cu:658-700); relu 0 = none, 1 = ReLU, 2 = clip(y, 0, 6).",
     "sniper_bn_stats": "Train-mode BatchNorm statistics -> mean, invstd, scale, shift and moving statistics (cuDNN convention, nn/cudnn/cudnn_batch_norm-inl.h).",
     "sniper_bn_apply_train": "BatchNorm(train) + Activation in one launch when the input statistics were accumulated by the producing conv's epilogue: finalisation (mean / invstd / scale / shift / moving statistics, nn/batch_norm.cu:658-700 semantics) folded into the apply pass.",
@@ -36,9 +35,7 @@ DOC = {
     "sniper_affine_relu_bwd": "Backward of relu?(x*scale+shift) for frozen BN.",
     "sniper_depthwise3x3_fwd": "Depthwise 3x3 convolution, pad 1, stride 1|2, NHWC, weights [9,C] fp32: Convolution(num_group = num_filter = C) of mobilenetv2_e2e.py:58-66 (src/operator/nn/depthwise_convolution-inl.h DepthwiseConvolutionOp::Forward).",
     "sniper_depthwise3x3_dgrad": "Data gradient of the depthwise convolution (depthwise_convolution-inl.h Backward, DepthwiseConv2dBackwardDataGpu), gather form.",
-    "sniper_depthwise3x3_wgrad_workspace_bytes": "Size of the caller-owned scratch one sniper_depthwise3x3_wgrad launch uses (the same for every shape).",
-    "sniper_depthwise3x3_set_wgrad_workspace": "Registers that scratch (caller-owned, no initialisation, must outlive later launches) for the weight-gradient launches on one (device, stream); the library itself never allocates device memory.",
-    "sniper_depthwise3x3_wgrad": "Weight gradient of the depthwise convolution (DepthwiseConv2dBackwardFilterGpu): dw[9,C] += per-channel correlation of dy with the shifted input; block partials summed in a fixed order through the registered scratch (bit-reproducible).",
+    "sniper_depthwise3x3_wgrad": "Weight gradient of the depthwise convolution (DepthwiseConv2dBackwardFilterGpu): dw[9,C] += per-channel correlation of dy with the shifted input; block partials summed in a fixed order through the slab of the stream's workspace (sniper_set_stream_workspace; bit-reproducible).",
     "sniper_im2col3x3s2_nchw": "im2col of MobileNetV2's first layer (3x3 / stride 2 / pad 1 over the 3-channel fp32 NCHW `data`, mobilenetv2_e2e.py:204-212) so that it runs on the wgmma GEMM; K order (kh, kw, ci), zero-padded to Kp.",
     "sniper_add_rows": "out = a + b on [M,C] rows: elemwise_add of the inverted-residual shortcut (mobilenetv2_e2e.py:22-24).",
     "sniper_relu_bwd": "dx = dy * (y > 0).",
