@@ -1,5 +1,6 @@
 """Host-side members of the path (numpy in / numpy out) over the C-ABI: chip sampling, NMS, overlaps.
-Mirrors lib/chips/chips.pyx, lib/nms/nms.py and lib/bbox of the reference (chip_generator / chip_worker: chip_worker.py)."""
+Mirrors lib/chips/chips.pyx, lib/nms/nms.py and lib/bbox of the reference (chip_generator / chip_worker: chip_worker.py),
+and the image reader the reference takes from OpenCV (`imread`, on PIL)."""
 import ctypes
 
 import numpy as np
@@ -62,3 +63,19 @@ def ignore_overlaps(boxes, query_boxes):
     out = np.zeros((b.shape[0], q.shape[0]), np.float64)
     check(lib().sniper_bbox_overlaps(_p(b), b.shape[0], _p(q), q.shape[0], _p(out), 1))
     return out
+
+
+def imread(path):
+    """cv2.imread(path, cv2.IMREAD_COLOR) on PIL: uint8 [H, W, 3] in BGR order.  Grayscale and palette images are
+    expanded to three channels, an alpha channel is dropped and the EXIF orientation is applied.  Raises OSError
+    naming the path when the file cannot be read or decoded (cv2.imread would return None)."""
+    try:
+        from PIL import Image, ImageOps
+    except ImportError as e:
+        raise ImportError("host.imread decodes images with Pillow (PIL), which is not installed") from e
+    try:
+        with Image.open(path) as im:
+            rgb = np.asarray(ImageOps.exif_transpose(im).convert('RGB'))
+    except OSError as e:
+        raise OSError("imread: cannot read image %s: %s" % (path, e)) from e
+    return np.ascontiguousarray(rgb[:, :, ::-1])

@@ -466,7 +466,9 @@ def default_config(neg=True, autofocus=False, network="resnet101", dataset="coco
     scales 1 / 2 / 4 / 8 / 12: 15 anchors; plain multi-scale inference without AutoFocus), for
     model_mnv2.SniperMobileNetV2.
     dataset="pascal_voc" (network "resnet101"): the blocks of configs/faster/sniper_res101_e2e_pascal_voc.yml instead,
-    for a 21-class SniperResNet101 evaluated by pascal_voc.PascalVOC."""
+    for a 21-class SniperResNet101 evaluated by pascal_voc.PascalVOC; its TRAIN block is the COCO yml's.
+    The roidb keys of load_data (TRAIN.FLIP, the FG / BG thresholds, TRAIN.BBOX_*, CLASS_AGNOSTIC and dataset.dataset,
+    the name load_data.load_proposal_roidb takes) have the same values in every shipped yml (:11, :116-172)."""
     import types
     S = types.SimpleNamespace
     if network == "resnet101":
@@ -488,7 +490,7 @@ def default_config(neg=True, autofocus=False, network="resnet101", dataset="coco
                  RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, RPN_MIN_SIZE=0)
     else:
         raise ValueError("default_config: network must be 'resnet101' or 'mobilenetv2', not %r" % (network,))
-    num_classes = 81
+    num_classes, name = 81, "coco"
     if dataset == "pascal_voc":
         if network != "resnet101":
             raise ValueError("default_config: the PASCAL VOC config is a ResNet-101 one, not %r" % (network,))
@@ -502,13 +504,17 @@ def default_config(neg=True, autofocus=False, network="resnet101", dataset="coco
                  VALID_RANGES=[(-1, 90), (32, 180), (75, -1)], AUTO_FOCUS=False, DO_PRUNING=[False, False, False],
                  CHIP_HYPERPARAMS=[(-1, -1, -1), (-1, -1, -1), (-1, -1, -1)], NMS=-1, NMS_SIGMA=0.55,
                  RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, RPN_MIN_SIZE=0)
-        num_classes = 21
+        num_classes, name = 21, "PascalVOC"
     elif dataset != "coco":
         raise ValueError("default_config: dataset must be 'coco' or 'pascal_voc', not %r" % (dataset,))
     return S(network=net,
              TRAIN=S(SCALES=[(1400, 2000), (800, 1280), (-1, 512)], VALID_RANGES=[(-1, 80), (32, 150), (120, -1)],
                      CPP_CHIPS=True, USE_NEG_CHIPS=neg, RPN_BATCH_SIZE=256, RPN_FG_FRACTION=0.5,
                      RPN_POSITIVE_OVERLAP=0.5, RPN_NEGATIVE_OVERLAP=0.4, BATCH_IMAGES=16, AUTO_FOCUS=autofocus,
-                     AUTO_FOCUS_DC_LOW=5, AUTO_FOCUS_SMALL_THRESH=64, AUTO_FOCUS_DC_HIGH=90),
+                     AUTO_FOCUS_DC_LOW=5, AUTO_FOCUS_SMALL_THRESH=64, AUTO_FOCUS_DC_HIGH=90, FLIP=True,
+                     FG_THRESH=0.5, BG_THRESH_HI=0.5, BG_THRESH_LO=0.0, BBOX_REGRESSION_THRESH=0.5,
+                     BBOX_NORMALIZATION_PRECOMPUTED=True, BBOX_MEANS=[0.0, 0.0, 0.0, 0.0],
+                     BBOX_STDS=[0.1, 0.1, 0.2, 0.2]),
              TEST=test,
-             dataset=S(NUM_CLASSES=num_classes))
+             CLASS_AGNOSTIC=True,
+             dataset=S(NUM_CLASSES=num_classes, dataset=name))

@@ -401,7 +401,7 @@ class Tester(object):
 
 
 def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device",
-                           imdb=None, detect_backend="host"):
+                           imdb=None, detect_backend="host", image_loader=None):
     """The CONCURRENT_JOBS == 1 path of imdb_detection_wrapper (:436-528): every scale of TEST.SCALES in turn (FocusChips
     of scale i feed scale i + 1 when DO_PRUNING[i + 1]), then the cross-scale aggregation.
     Returns (all_boxes[class][image], stats) with per-scale chip counts / detect / post-processing seconds, the NMS
@@ -410,7 +410,8 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
     dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
     and its seconds to stats['eval_s'].  `net` is a `DetectionNetwork`; config is the network's own (e.g.
-    iterator.default_config(network="mobilenetv2") for a SniperMobileNetV2): its RPN_FEAT_STRIDE must be the net's."""
+    iterator.default_config(network="mobilenetv2") for a SniperMobileNetV2): its RPN_FEAT_STRIDE must be the net's.
+    image_loader(path) decodes the entries without 'image_data' (e.g. host.imread)."""
     T = config.TEST
     if int(config.network.RPN_FEAT_STRIDE) != int(net.feat_stride):
         raise ValueError("imdb_detection_wrapper: config.network.RPN_FEAT_STRIDE is %s, the network's stride is %s"
@@ -420,7 +421,7 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     detections, stats = [], dict(scales=[])
     nb = batch_images or list(T.BATCH_IMAGES)
     for scale_i, (nbatch, scale) in enumerate(zip(nb, T.SCALES)):
-        it = MNIteratorTestAutoFocus(roidb, config, scale, batch_size=nbatch, device=device)
+        it = MNIteratorTestAutoFocus(roidb, config, scale, batch_size=nbatch, device=device, image_loader=image_loader)
         tester = Tester(net, None, roidb, it, config, batch_size=nbatch, num_classes=num_classes)
         t0 = time.time()
         dets, maps = tester.get_detections(do_pruning=bool(T.DO_PRUNING[scale_i]), autofocus=bool(T.AUTO_FOCUS),
@@ -453,16 +454,18 @@ def proposal_file_name(config):
     return '{}_{}_rpn.pkl'.format(config.dataset.dataset.upper(), config.dataset.test_image_set)
 
 
-def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0"):
+def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0",
+                                     image_loader=None):
     """The CONCURRENT_JOBS == 1 path of imdb_proposal_extraction_wrapper (:559-610): RPN proposals of every image at every
     scale of TEST.SCALES (`net.forward_rpn`), each image's rows stacked in scale order, pickled as a list of float32
     [n, 5] arrays to save_path/proposal_file_name(config) (protocol 2, readable by the reference's Python 2).  Returns
-    (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds."""
+    (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds.  image_loader(path)
+    decodes the entries without 'image_data' (e.g. host.imread)."""
     T = config.TEST
     proposals, stats = [], dict(scales=[])
     nb = batch_images or list(T.BATCH_IMAGES)
     for nbatch, scale in zip(nb, T.SCALES):
-        it = MNIteratorTest(roidb, config, scale, batch_size=nbatch, device=device)
+        it = MNIteratorTest(roidb, config, scale, batch_size=nbatch, device=device, image_loader=image_loader)
         tester = Tester(net, None, roidb, it, config, batch_size=nbatch, num_classes=1)
         t0 = time.time()
         proposals.append(tester.extract_proposals(n_proposals=n_proposals))
