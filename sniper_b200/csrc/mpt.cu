@@ -232,16 +232,18 @@ struct NmsArgs {
   const int32_t* fast_keep;      // optional results of mpt_nms_fast_kernel: [B,1024], [B], [B]
   const int32_t* fast_nkept;
   const int32_t* fast_fallback;
+  int index_ties;          // 1: equal scores are kept in ascending row order (MultiProposal); 0: the reference's scan order
 };
 
 constexpr int kNmsThreads = 1024;
 
 // ------------------------------------------------------------------------------------------------
 // Fast path of the greedy NMS: two-level score histogram -> top <= 4096 candidates -> exact bitonic sort ->
-// trips of <= 64 candidates resolved with IoU bit masks (ballot / shuffle reductions) by one thread that
-// also replays the reference's row swaps, so exact score ties are broken in the reference's scan order
-// (lexicographic (d%32, (d%1024)/32, d/1024) of the candidate's current row distance d to the front).
-// It falls back (flag) to the round-by-round emulation in mpt_nms_assign_kernel when a run of equal scores
+// trips of <= 64 candidates resolved with IoU bit masks (ballot / shuffle reductions) by one thread.  Exact score
+// ties: with index_ties (the inference operator) in ascending row order, i.e. the sorted order of the (score, row)
+// keys; otherwise (MultiProposalTarget) the thread replays the reference's row swaps, so ties are broken in the
+// reference's scan order (lexicographic (d%32, (d%1024)/32, d/1024) of the candidate's current row distance d to
+// the front).  It falls back (flag) to the round-by-round emulation in mpt_nms_assign_kernel when a run of equal scores
 // is longer than a trip, when more than 4096 candidates share the boundary sub-bin, or when the selection
 // is exhausted before R boxes are kept while unselected valid candidates remain.
 constexpr int kFastCap = 4096;          // candidates sorted per chip
@@ -257,6 +259,7 @@ struct FastArgs {
   int32_t* nkept;      // [B]
   int32_t* fallback;   // [B]
   OverlapMap omap;
+  int index_ties;      // as NmsArgs::index_ties
 };
 
 __device__ __forceinline__ int score_bin(float s) {
@@ -451,7 +454,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) mpt_nms_fast_kernel(FastArgs p
     for (int off = 8; off > 0; off >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, off);
     if (sub == 0) { s_mask[grp] = m; s_alive[grp] = alive ? 1 : 0; }
     __syncthreads();
-    // (c) sequential resolve by one thread, replaying the reference's swaps for its tie order
+    // (c) sequential resolve by one thread; the swaps are replayed for the reference's tie order (index_ties = 0)
     if (t == 0) {
       unsigned long long removed = 0;   // suppressed or already selected
       int k = nk;
@@ -466,7 +469,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) mpt_nms_fast_kernel(FastArgs p
           for (int c = i; c < e; ++c) {
             if (!s_alive[c] || ((removed >> c) & 1ull)) continue;
             const unsigned d = (unsigned)((int)s_pos[base + c] - k);   // row distance to the front (row k)
-            const unsigned key = ((d & 31u) << 10) | (((d >> 5) & 31u) << 5) | (d >> 10);
+            const unsigned key = p.index_ties ? (unsigned)c : ((d & 31u) << 10) | (((d >> 5) & 31u) << 5) | (d >> 10);
             if (key < bestkey) { bestkey = key; best = c; }
           }
           if (best < 0) break;
@@ -510,7 +513,10 @@ __global__ void __launch_bounds__(kNmsThreads, 1) mpt_nms_fast_kernel(FastArgs p
 // One CTA per chip.  Positions 0..AHW-1 hold (score, id) in shared memory; the reference's row swap
 // (cu:178-199) becomes a 6-byte swap here, the 16-byte boxes never move.  Tie order of the
 // reference's three-level strided argmax (cu:139-176) == lexicographic (lane, warp, stride index)
-// among equal scores, which is what the packed 64-bit key below encodes.
+// among equal scores, which is what the packed 64-bit key below encodes.  With index_ties the lowest
+// row id wins a tie instead (the inference operator), and the low bits only carry the position.  kIndexTies ==
+// p.index_ties, a template parameter so that the training operator's scan is not slowed by the tie test.
+template <bool kIndexTies>
 __global__ void __launch_bounds__(kNmsThreads, 1) mpt_nms_assign_kernel(NmsArgs p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* s_score = reinterpret_cast<float*>(smem_raw);
@@ -545,23 +551,26 @@ __global__ void __launch_bounds__(kNmsThreads, 1) mpt_nms_assign_kernel(NmsArgs 
       int i = 0;
       for (int pos = j + t; pos < AHW; pos += kNmsThreads, ++i) {
         const float s = s_score[pos];
-        if (s > best) {
+        if (s > best || (kIndexTies && s == best && s_id[pos] < bestid)) {
           best = s;
           besti = i;
           bestid = s_id[pos];
         }
       }
     }
-    unsigned long long key = ((unsigned long long)ord_desc(best) << 32) |
-                             ((unsigned long long)((lane << 26) | (warp << 21) | (besti << 16) | bestid));
+    // index_ties: id (15 bits, AHW <= 32768) | stride index (5) | thread (10); else lane | warp | stride index | id
+    const uint32_t lo_key = kIndexTies ? (bestid << 15) | (besti << 10) | (uint32_t)t
+                                       : (lane << 26) | (warp << 21) | (besti << 16) | bestid;
+    unsigned long long key = ((unsigned long long)ord_desc(best) << 32) | lo_key;
     key = warp_min_u64(key);
     if (lane == 0) s_warpkey[warp] = key;
     __syncthreads();
     key = warp_min_u64(s_warpkey[lane]);
     const uint32_t lo = (uint32_t)key;
     const float sel_score = ord_desc_inv((uint32_t)(key >> 32));
-    const int sel_id = lo & 0xffff;
-    const int m = j + (int)(((lo >> 21) & 31) * 32 + (lo >> 26)) + (int)((lo >> 16) & 31) * kNmsThreads;
+    const int sel_id = kIndexTies ? (int)(lo >> 15) : (int)(lo & 0xffff);
+    const int m = j + (kIndexTies ? (int)(lo & 1023) + (int)((lo >> 10) & 31) * kNmsThreads
+                                  : (int)(((lo >> 21) & 31) * 32 + (lo >> 26)) + (int)((lo >> 16) & 31) * kNmsThreads);
     if (sel_score == -1.0f) break;  // cu:214-216 (uniform across the block)
     if (t == 0) s_keep[vct] = sel_id;
     vct++;
@@ -900,7 +909,7 @@ static int nms_assign_launch(const float* boxes, const float* score, const float
                              float* rois, float* label, float* bbox_target, float* bbox_weight,
                              int32_t* keep_idx, int32_t* num_kept, int do_assign, int32_t* fast_scratch,
                              void* stream, const int32_t* id_map = nullptr, float* score_out = nullptr,
-                             long filler_stride = 0, const OverlapMap* omap = nullptr) {
+                             long filler_stride = 0, const OverlapMap* omap = nullptr, int index_ties = 0) {
   SN_CHECK(AHW >= R, "nms: anchors per chip (%d) < post_nms_top_n (%d)", AHW, R);
   SN_CHECK(AHW <= 32768, "nms: anchors per chip (%d) > 32768", AHW);
   SN_CHECK(R <= 1024, "nms: post_nms_top_n (%d) > 1024", R);
@@ -912,11 +921,13 @@ static int nms_assign_launch(const float* boxes, const float* score, const float
   n.bbox_weight = bbox_weight; n.keep_idx = keep_idx; n.num_kept = num_kept; n.do_assign = do_assign;
   n.id_map = id_map; n.score_out = score_out; n.filler_stride = filler_stride > 0 ? filler_stride : AHW;
   if (omap) n.omap = *omap; else { memset(&n.omap, 0, sizeof(n.omap)); }
+  n.index_ties = index_ties;
   const size_t smem = (size_t)AHW * 6 + 16;
   static bool attr_set = false;
   const size_t fast_smem = (size_t)kFastCap * (8 + 16 + 4 + 2) + kFastBins * 4 + 1024 * (20 + 2) + 64 * 8 + 64 * 4 + 64;
   if (!attr_set) {
-    SN_CUDA(cudaFuncSetAttribute(mpt_nms_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    SN_CUDA(cudaFuncSetAttribute(mpt_nms_assign_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    SN_CUDA(cudaFuncSetAttribute(mpt_nms_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     SN_CUDA(cudaFuncSetAttribute(mpt_nms_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set = true;
   }
@@ -926,11 +937,15 @@ static int nms_assign_launch(const float* boxes, const float* score, const float
     f.boxes = n.boxes; f.scores = score; f.areas = area; f.AHW = AHW; f.R = R; f.nms_thresh = nms_thresh;
     f.keep_ids = fast_scratch; f.nkept = fast_scratch + (size_t)B * 1024; f.fallback = f.nkept + B;
     f.omap = n.omap;
+    f.index_ties = index_ties;
     mpt_nms_fast_kernel<<<B, kNmsThreads, fast_smem, (cudaStream_t)stream>>>(f);
     SN_LAUNCH_CHECK();
     n.fast_keep = f.keep_ids; n.fast_nkept = f.nkept; n.fast_fallback = f.fallback;
   }
-  mpt_nms_assign_kernel<<<B, kNmsThreads, smem, (cudaStream_t)stream>>>(n);
+  if (index_ties)
+    mpt_nms_assign_kernel<true><<<B, kNmsThreads, smem, (cudaStream_t)stream>>>(n);
+  else
+    mpt_nms_assign_kernel<false><<<B, kNmsThreads, smem, (cudaStream_t)stream>>>(n);
   SN_LAUNCH_CHECK();
   return 0;
 }
@@ -976,6 +991,8 @@ size_t sniper_multi_proposal_workspace_bytes(int B, int A, int H, int W, int pre
 // the anchors of its precomputed anchor-overlap map, roi_iou_thresh; .cu:267-387) instead of the exact NMS of the CPU op.
 // Rows after the kept ones are rand() boxes in the reference; here the deterministic filler of the training operator
 // with score 0.  keep_idx / num_kept: optional parity outputs (original anchor indices).
+// Equal scores are taken in ascending anchor index, by the selection and by both NMS kernels (the reference sorts with
+// std::sort / nth_element, whose order of equal scores is unspecified; the compacted rows keep the index order).
 int sniper_multi_proposal_fwd(const float* cls_prob, const float* bbox_pred, const float* im_info, int B, int A, int H,
                               int W, int pre_nms_top_n, int post_nms_top_n, int feat_stride, const float* scales, int ns,
                               const float* ratios, int nr, float nms_thresh, int flags, float roi_iou_thresh, int layout,
@@ -1036,7 +1053,7 @@ int sniper_multi_proposal_fwd(const float* cls_prob, const float* bbox_pred, con
   }
   return nms_assign_launch(boxes, score, area, nullptr, nullptr, B, K, 0, post_nms_top_n, nms_thresh, rois, nullptr,
                            nullptr, nullptr, keep_idx, num_kept, 0, nms_fast_enabled() ? fast_scratch : nullptr, stream,
-                           id_map, scores, (long)AHW, &om);
+                           id_map, scores, (long)AHW, &om, 1);
 }
 
 }  // extern "C"

@@ -59,11 +59,17 @@ def generate_anchors(feat_stride, scales, ratios):
 
 def multi_proposal(cls_prob, bbox_pred, im_info, *, feat_stride=16, scales=(2, 4, 7, 10, 13, 16, 24),
                    ratios=(0.5, 1, 2), rpn_pre_nms_top_n=12000, rpn_post_nms_top_n=300, threshold=0.7,
-                   suppress_anchor_types=False, fast_nms=False, roi_iou_thresh=0.3, layout=NCHW, return_keep=False):
+                   suppress_anchor_types=False, fast_nms=False, roi_iou_thresh=0.3, layout=NCHW, return_keep=False,
+                   return_fallback=False):
     """MultiProposal forward -- the inference proposal operator (multi_proposal.cc:273-374 semantics: decode, min-size
     filter, the rpn_pre_nms_top_n best anchors, greedy NMS), on device; suppress_anchor_types / fast_nms select the two
     extras of the reference's GPU build (multi_proposal.cu:505-508, 267-387).  Returns rois [B*R,5], scores [B*R]
-    (+ keep_idx [B*R] original anchor indices / -1 for filler rows, num_kept [B])."""
+    (+ keep_idx [B*R] original anchor indices / -1 for filler rows, num_kept [B]; + the per-image flag of the bit-mask
+    NMS, 1 = the sequential kernel ran, meaningful unless SNIPER_NMS_FAST=0).
+
+    Equal scores are taken in ascending anchor index, by the pre-NMS selection and by the NMS: the rule of the oracle
+    (oracle/mp_cpuop.c), since the reference sorts with std::sort, whose order of equal scores is unspecified.  The
+    training operator, multi_proposal_target, breaks NMS ties in the reference GPU kernel's scan order instead."""
     _f32(cls_prob), _f32(bbox_pred), _f32(im_info)
     A = len(scales) * len(ratios)
     if layout == NCHW:
@@ -90,6 +96,14 @@ def multi_proposal(cls_prob, bbox_pred, im_info, *, feat_stride=16, scales=(2, 4
         len(s), rp, len(r), float(threshold), (1 if suppress_anchor_types else 0) | (2 if fast_nms else 0),
         float(roi_iou_thresh), layout, sc, dc, _ptr(rois),
         _ptr(scores), _ptr(keep), _ptr(nkept), _ptr(ws), ws_bytes, _stream()))
+    if return_fallback:
+        # per-image flag written by mpt_nms_fast_kernel after the workspace's decoded and compacted rows (16-byte
+        # aligned arrays, sniper_multi_proposal_fwd)
+        r16 = lambda n: (n + 15) // 16 * 16
+        total, K = B * A * H * W, B * min(int(rpn_pre_nms_top_n), A * H * W)
+        off = 16 * total + 2 * r16(4 * total) + 16 * K + 3 * r16(4 * K)
+        fb = ws[off:off + B * 1026 * 4].view(torch.int32)[B * 1025:B * 1026].clone()
+        return rois, scores, keep, nkept, fb
     if return_keep:
         return rois, scores, keep, nkept
     return rois, scores

@@ -348,6 +348,35 @@ def test_inference_op_restatement_is_bit_identical_to_the_reference_cpu_operator
         assert (scores[b * 300 + k:(b + 1) * 300] == 0).all()       # the reference's filler rows carry score 0
 
 
+@pytest.mark.parametrize("name", ["resnet101-s0-landscape", "resnet101-s0-portrait", "resnet101-largest-tie_free",
+                                  "mobilenetv2-s0-landscape", "mobilenetv2-s0-portrait"])
+def test_inference_op_restatement_matches_the_reference_at_tester_canvases(name):
+    """The same pin at the Tester's canvases (tests/multi_proposal_cases.py, tie-free scores): rectangular maps in both
+    orientations, several images with their own im_info smaller than the canvas, the ResNet-101 anchors at stride 16
+    (up to 225792 anchors per image) and the MobileNetV2 anchors at stride 32 with 6000 pre-NMS rows.  The reference
+    operator always sorts min(12000, A*H*W) rows (multi_proposal.cc:176); the 6000-row cases are compared where that
+    cannot matter, which the oracle itself shows: its 300 rows are the same with 6000 and with 12000."""
+    import multi_proposal_cases as C
+    c = C.build(name)
+    assert c["regime"] == "tie_free" and c["flags"] == 0
+    cls_prob, bbox_pred, im_info, pre = c["cls_prob"], c["bbox_pred"], c["im_info"], c["pre"]
+    rois, scores = _need_ref(O.ref_multi_proposal(cls_prob, bbox_pred, im_info, pre=pre, **c["kw"]))
+    mine = O.multi_proposal(cls_prob, bbox_pred, im_info, pre=pre, libm_exp=True, **c["kw"])
+    if pre < 12000:
+        wide = O.multi_proposal(cls_prob, bbox_pred, im_info, pre=12000, libm_exp=True, **c["kw"])
+        assert all(mine[k].tobytes() == wide[k].tobytes() for k in ("rois", "scores", "keep_idx"))
+    B = len(im_info)
+    assert B >= 2 and c["H"] != c["W"] and (im_info[:, 0] != im_info[:, 1]).all()
+    for b in range(B):
+        k = int(mine["num_kept"][b])
+        assert k > 50
+        sl = slice(b * 300, b * 300 + k)
+        assert mine["rois"][sl].tobytes() == rois[sl].tobytes(), b
+        assert mine["scores"][sl].tobytes() == scores[sl].tobytes(), b
+        assert (scores[b * 300 + k:(b + 1) * 300] == 0).all()
+        assert (rois[sl, 3] <= im_info[b, 1] - 1).all() and (rois[sl, 4] <= im_info[b, 0] - 1).all()
+
+
 def test_inference_op_gpu_build_extras():
     """The two extras of multi_proposal.cu (pinned by the .cu text only): anchor-type suppression removes exactly the
     anchor types (i+4)%7==0 / (i+2)%7==0 from the output; FastNMS keeps a superset-or-equal of rows early in the list
