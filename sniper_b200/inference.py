@@ -2,15 +2,16 @@
 bookkeeping): per-chip box decoding (`Tester.detect`, :100-139), score thresholding (`get_detections`, :291-301) and the
 cross-scale aggregation with per-(image, class) soft-NMS (`Tester.aggregate`, :152-230).
 
-The reference aggregates on the host and farms the NMS out to `Pool(32)` processes, one `cpu_soft_nms` call per image
-and class; here every (image, class) problem of the run is ONE launch of `sniper_soft_nms_batched`.  `backend="host"`
-runs the same code path through the C-ABI host `sniper_cpu_soft_nms` (bit-identical to the reference's Cython) -- the
-parity tests compare the two.
+Two detection backends feed the aggregation; they differ only in where rows are decoded and thresholded.  The host one
+(`detect_postprocess`, `threshold_detections`, nested lists per class / image / chip) is the reference's arithmetic in
+numpy and the oracle of the other.  The device one keeps every detection on the GPU: `ops.detect_post` appends each
+batch's surviving rows with their `pack_key` order key to a `DeviceDetections` run buffer.
 
-Two detection backends feed the aggregation.  The host one (`detect_postprocess`, `threshold_detections`, nested lists
-per class / image / chip) is the reference's arithmetic in numpy and the oracle of the other.  The device one keeps
-every detection on the GPU: `ops.detect_post` appends each batch's surviving rows to a `DeviceDetections` run buffer,
-and `aggregate` sorts the run by `pack_key` and cuts it into the soft-NMS problems without a host round trip.
+`aggregate` reduces either to float32 rows and an (image, class) problem index per scale, and from there has one path:
+a stable sort by problem, segment offsets, the soft-NMS, the MAX_PER_IMAGE cut.  The reference farms the NMS out to
+`Pool(32)` processes, one `cpu_soft_nms` call per image and class; here every problem of the run is ONE launch of
+`sniper_soft_nms_batched`.  `backend="host"` runs the C-ABI host `sniper_cpu_soft_nms` (bit-identical to the
+reference's Cython) per problem instead -- the parity tests compare the two.
 Not built (needs OpenCV, absent from this image): FocusChip generation
 (`lib/chips/chips_inference.py`: cv2.dilate + findContours).
 """
@@ -218,91 +219,70 @@ class DeviceDetections(object):
         return self.rows[:n], self.keys[:n]
 
 
-def _device_problems(dets, num_images, num_classes):
-    """The runs of every scale -> (flat [n,5] device rows sorted into the soft-NMS problems, int32 offsets [nprob+1])."""
-    parts = [d.result() for d in dets]
-    rows = torch.cat([r for r, _ in parts], 0)
-    keys = torch.cat([k for _, k in parts], 0)
+def _run_problems(dets, num_classes):
+    """One scale's `DeviceDetections` -> (rows [n,5], int64 problem index image * (K - 1) + class - 1 [n]) on its
+    device, sorted by key: image, class, chip, roi."""
+    rows, keys = dets.result()
     keys, order = torch.sort(keys, stable=True)
-    rows = rows[order].contiguous()
     shift = _ROI_BITS + _CHIP_BITS + _SCALE_BITS
-    prob = (keys >> (shift + _CLASS_BITS)) * (num_classes - 1) + ((keys >> shift) & ((1 << _CLASS_BITS) - 1)) - 1
-    nprob = num_images * (num_classes - 1)
-    if rows.shape[0] and (int(prob[0]) < 0 or int(prob[-1]) >= nprob):
-        raise ValueError("aggregate: detections of an image or class outside %d images x %d classes"
-                         % (num_images, num_classes))
-    offsets = torch.searchsorted(prob, torch.arange(nprob + 1, device=prob.device)).to(torch.int32)
-    return rows, offsets
+    cls = (keys >> shift) & ((1 << _CLASS_BITS) - 1)
+    return rows[order], (keys >> (shift + _CLASS_BITS)) * (num_classes - 1) + cls - 1
+
+
+def _list_problems(all_cls_dets, valid_range, num_images, num_classes, device):
+    """One scale's nested lists all_cls_dets[j][i][chip] -> (rows [n,5], int64 problem index [n]) on `device`, stacked
+    class by class, image by image, chip by chip, through the scale's valid range (the area rule of
+    `_valid_range_filter`)."""
+    blocks, prob = [np.zeros((0, 5), np.float32)], [0]
+    for j in range(1, num_classes):
+        for i in range(num_images):
+            for cls_dets in all_cls_dets[j][i]:
+                blocks.append(np.asarray(cls_dets, np.float32).reshape(-1, 5))
+                prob.append(i * (num_classes - 1) + j - 1)
+    d = np.concatenate(blocks, 0)
+    p = np.repeat(np.array(prob, np.int64), [len(b) for b in blocks])
+    areas = (d[:, 3] - d[:, 1]) * (d[:, 2] - d[:, 0])
+    keep = np.ones(len(d), bool)
+    if valid_range[0] > 0:
+        keep &= areas > valid_range[0] * valid_range[0]
+    if valid_range[1] > 0:
+        keep &= areas <= valid_range[1] * valid_range[1]
+    return torch.from_numpy(d[keep]).to(device), torch.from_numpy(p[keep]).to(device)
 
 
 def aggregate(scale_cls_dets, valid_ranges, num_images, num_classes, sigma=0.55, nms_thresh=0.3, max_per_image=100,
               backend="device", device="cuda"):
     """Tester.aggregate (:152-230).  scale_cls_dets[s][j][i] = list over chips of [n,5] detections of class j in image i
-    at scale s.  Returns all_boxes[j][i] = [n,5] after the valid-range filter, Gaussian soft-NMS (sigma, threshold
-    0.001; nms_worker -> nms_wrapper -> cpu_soft_nms) and the MAX_PER_IMAGE cut.
-    With one `DeviceDetections` per scale instead (their rows passed the valid range in `ops.detect_post`), the
-    problems are cut on the device: one stable sort by key, segment offsets, the same soft-NMS launch, one copy back."""
+    at scale s, or one `DeviceDetections` per scale (its rows passed the valid range in `ops.detect_post`).  Returns
+    all_boxes[j][i] = [n,5] after the valid-range filter, Gaussian soft-NMS (sigma, threshold 0.001; nms_worker ->
+    nms_wrapper -> cpu_soft_nms) and the MAX_PER_IMAGE cut.
+    Every scale's rows are tagged with their (image, class) problem; one stable sort by problem then stacks a problem's
+    rows in the (scale, chip, row) order of the reference's nested loops.  The sort runs where the rows are: on the
+    device for `DeviceDetections`, or for nested lists with backend="device"; on the CPU otherwise."""
     assert len(scale_cls_dets) == len(valid_ranges), 'A valid range should be specified for each test scale'
     on_device = [isinstance(d, DeviceDetections) for d in scale_cls_dets]
     if any(on_device):
         if not all(on_device):
             raise TypeError("aggregate: every scale's detections must come from the same backend (got nested lists "
                             "and DeviceDetections)")
-        flat, offsets = _device_problems(scale_cls_dets, num_images, num_classes)
-        if backend == "device" and flat.shape[0]:
-            out, counts = ops.soft_nms_batched(flat, offsets, sigma=sigma, Nt=nms_thresh, threshold=0.001, method=2)
-            out, counts, offsets = out.cpu().numpy(), counts.cpu().numpy(), offsets.cpu().numpy()
-            final = [out[offsets[p]:offsets[p] + counts[p]] for p in range(len(counts))]
-        else:
-            final = [host.cpu_soft_nms(p.copy(), sigma=sigma, Nt=nms_thresh, threshold=0.001, method=2) if len(p) else p
-                     for p in np.split(flat.cpu().numpy(), offsets.cpu().numpy()[1:-1])]
-        return _per_image(final, num_images, num_classes, max_per_image)
-    # Gather every detection of the run once, tagged with its (image, class) problem, apply each scale's valid range to
-    # the whole block, and cut the (stably) sorted block into the per-problem arrays: rows of a problem keep the
-    # (scale, chip, row) order in which the reference's nested loops stack them.
-    blocks, keys = [], []
-    for all_cls_dets, vr in zip(scale_cls_dets, valid_ranges):
-        sb, sk = [], []
-        for j in range(1, num_classes):
-            for i in range(num_images):
-                for cls_dets in all_cls_dets[j][i]:
-                    d = np.asarray(cls_dets, np.float32).reshape(-1, 5)
-                    if d.shape[0]:
-                        sb.append(d)
-                        sk.append(np.full(d.shape[0], i * (num_classes - 1) + (j - 1), np.int64))
-        if sb:
-            d, k = np.concatenate(sb, 0), np.concatenate(sk)
-            areas = (d[:, 3] - d[:, 1]) * (d[:, 2] - d[:, 0])          # as _valid_range_filter (no +1)
-            keep = np.ones(len(d), bool)
-            if vr[0] > 0:
-                keep &= areas > vr[0] * vr[0]
-            if vr[1] > 0:
-                keep &= areas <= vr[1] * vr[1]
-            blocks.append(d[keep])
-            keys.append(k[keep])
-    nprob = num_images * (num_classes - 1)
-    if blocks:
-        d, k = np.concatenate(blocks, 0), np.concatenate(keys)
-        order = np.argsort(k, kind="stable")
-        d, k = np.ascontiguousarray(d[order]), k[order]
-        cuts = np.searchsorted(k, np.arange(1, nprob))
-        problems = np.split(d, cuts)
+        parts = [_run_problems(d, num_classes) for d in scale_cls_dets]
     else:
-        problems = [np.zeros((0, 5), np.float32) for _ in range(nprob)]
-    if backend == "device":
-        sizes = [len(p) for p in problems]
-        offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int32)
-        flat = np.concatenate(problems, 0) if sum(sizes) else np.zeros((0, 5), np.float32)
-        if len(flat):
-            out, counts = ops.soft_nms_batched(torch.from_numpy(flat).to(device), torch.from_numpy(offsets).to(device),
-                                               sigma=sigma, Nt=nms_thresh, threshold=0.001, method=2)
-            out, counts = out.cpu().numpy(), counts.cpu().numpy()
-        else:
-            out, counts = flat, np.zeros(len(problems), np.int32)
-        final = [out[offsets[p]:offsets[p] + counts[p]] for p in range(len(problems))]
+        dev = device if backend == "device" else "cpu"
+        parts = [_list_problems(d, vr, num_images, num_classes, dev) for d, vr in zip(scale_cls_dets, valid_ranges)]
+    prob, order = torch.sort(torch.cat([p for _, p in parts]), stable=True)
+    rows = torch.cat([r for r, _ in parts], 0)[order]
+    nprob = num_images * (num_classes - 1)
+    if rows.shape[0] and (int(prob[0]) < 0 or int(prob[-1]) >= nprob):
+        raise ValueError("aggregate: detections of an image or class outside %d images x %d classes"
+                         % (num_images, num_classes))
+    offsets = torch.searchsorted(prob, torch.arange(nprob + 1, device=prob.device)).to(torch.int32)
+    if backend == "device" and rows.shape[0]:
+        out, counts = ops.soft_nms_batched(rows, offsets, sigma=sigma, Nt=nms_thresh, threshold=0.001, method=2)
+        out, counts, offsets = out.cpu().numpy(), counts.cpu().numpy(), offsets.cpu().numpy()
+        final = [out[offsets[p]:offsets[p] + counts[p]] for p in range(len(counts))]
     else:
         final = [host.cpu_soft_nms(p.copy(), sigma=sigma, Nt=nms_thresh, threshold=0.001, method=2) if len(p) else p
-                 for p in problems]
+                 for p in np.split(rows.cpu().numpy(), offsets.cpu().numpy()[1:-1])]
     return _per_image(final, num_images, num_classes, max_per_image)
 
 

@@ -12,7 +12,8 @@ Host-side mirror of `lib/iterators/MNIteratorTestAutoFocus.py` (:13-141), `lib/i
                                                         backend="device" one `sniper_detect_post` launch per batch into
                                                         a device run buffer (no detection crosses to the host before
                                                         the soft-NMS has run)
-  per-(image, class) cpu_soft_nms in a Pool(32)         ONE `sniper_soft_nms_batched` launch for the whole run
+  per-(image, class) cpu_soft_nms in a Pool(32)         `inference.aggregate`, one path for both backends: ONE
+                                                        `sniper_soft_nms_batched` launch for the whole run
   FocusChips with OpenCV                                `chips_inference.add_chips`
 
 The proposal extraction of main_test.py with TEST.EXTRACT_PROPOSALS -- `MNIteratorTest`, `Tester.get_proposals` /
@@ -315,15 +316,15 @@ class Tester(object):
         B = batch['data'].shape[0]
         scores, preds = inference.detect_postprocess(rois.cpu().numpy(), cls_prob.cpu().numpy(), deltas.cpu().numpy(),
                                                      batch['im_info'].cpu().numpy(), B)
-        maps = []
-        if want_map:
-            fm = out[4].cpu().numpy()
-            info = batch['im_info'].cpu().numpy()
-            s = float(self.net.feat_stride)
-            for idx in range(B):       # the map of the chip itself (the canvas is padded to the batch maximum)
-                mh, mw = int(math.ceil(info[idx, 0] / s)), int(math.ceil(info[idx, 1] / s))
-                maps.append(fm[idx, :mh, :mw].copy())
+        maps = self._chip_maps(out[4].cpu().numpy(), batch['im_info'].cpu().numpy()) if want_map else []
         return scores, preds, batch, batch['im_ids'], maps, batch['chip_ids']
+
+    def _chip_maps(self, fm, im_info):
+        """The FocusPixel map of each chip of a batch: fm [B,H,W] covers the canvas, which is padded to the batch
+        maximum, so chip idx's own map is its first ceil(resized height / stride) x ceil(resized width / stride) cells."""
+        s = float(self.net.feat_stride)
+        return [fm[idx, :int(math.ceil(im_info[idx, 0] / s)), :int(math.ceil(im_info[idx, 1] / s))].copy()
+                for idx in range(fm.shape[0])]
 
     def get_detections(self, cls_thresh=1e-3, cache_name='cache', evaluate=False, vis=False, vis_path=None,
                        do_pruning=False, autofocus=False, vis_ext='.png', backend="host", scale_index=0):
@@ -382,12 +383,9 @@ class Tester(object):
         dets.finish()
         self.detect_time += time.time() - t0
         t0 = time.time()
-        s = float(self.net.feat_stride)
         for fm, info, im_ids, chip_ids in staged:
-            fm, info = fm.numpy(), info.numpy()
-            for idx, (im_id, chip_id) in enumerate(zip(im_ids, chip_ids)):
-                mh, mw = int(math.ceil(info[idx, 0] / s)), int(math.ceil(info[idx, 1] / s))
-                all_maps[im_id][chip_id] = (None, fm[idx, :mh, :mw].copy())
+            for m, im_id, chip_id in zip(self._chip_maps(fm.numpy(), info.numpy()), im_ids, chip_ids):
+                all_maps[im_id][chip_id] = (None, m)
         self.post_time += time.time() - t0
         return dets, all_maps
 
