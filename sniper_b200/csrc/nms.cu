@@ -5,74 +5,85 @@
 // nms_worker.worker) -- the "per-scale NMS latency" of BASELINE config 5.  One CTA per problem; all problems of a scale
 // (images x 80 classes) run in one launch.
 //
-// Semantics of the reference loop, restated order-free: repeat { take the highest-scoring remaining box (rows the
-// reference has swapped to the front are exactly the boxes taken so far, in order); multiply the score of every other
-// remaining box by w(IoU with it); drop boxes whose score falls below `threshold` }.  The output rows are the taken boxes
-// in the order taken, each with the score it had when taken = the reference's returned array.  Arithmetic follows the
-// Cythonized reference (float IoU with the `+ 1` sums evaluated in double and narrowed once, Gaussian weight =
-// exp evaluated in double); this file is compiled with -fmad=false.  Exact score ties are broken by the lower input row
-// (the reference breaks them by its current, swap-dependent order).
+// The kernel runs the reference loop on the reference's own row array, in parallel within each step.  Positions
+// [i, live) of `work` hold the remaining rows, as boxes[i:N] do in the reference.  Take i: among them the highest
+// score, the lowest position on exact ties (the reference's strict `<` scan from i); it swaps places with the row at
+// position i.  Decay: every row at a position above i, each once against the taken box; a row whose score falls below
+// `threshold` is removed.  Whether a row survives does not depend on its position, so the reference's swap-with-last
+// compaction, which interleaves with its decay, can be replayed after the round: with M survivors at positions i+1 ..
+// live-1, those below i+1+M stay, the h-th hole of [i+1, i+1+M) counting up receives the h-th survivor at >= i+1+M
+// counting down from the end, and live becomes i+1+M.  So exact score ties go where the reference sends them, and
+// positions [0, live) at the end are the reference's returned array.  Arithmetic follows the Cythonized reference
+// (float IoU with the `+ 1` sums evaluated in double and narrowed once, Gaussian weight = exp evaluated in double);
+// this file is compiled with -fmad=false.
 #include "common.cuh"
+#include <limits.h>
 #include <math.h>
 
 namespace {
 
 constexpr int kNmsTPB = 256;
+constexpr int kNmsWarps = kNmsTPB / 32;
 
 __global__ void __launch_bounds__(kNmsTPB) soft_nms_batched_kernel(float* __restrict__ dets, const int* __restrict__ offsets,
                                                                    float sigma, float Nt, float threshold,
                                                                    unsigned method, int* __restrict__ out_counts,
                                                                    float* __restrict__ scratch) {
-  const int p = blockIdx.x;
+  const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int base = offsets[p], N = offsets[p + 1] - base;
   float* d = dets + (size_t)base * 5;
-  float* work = scratch + (size_t)base * 5;     // the remaining boxes (score < 0 marks a removed / taken row)
-  __shared__ float s_val[kNmsTPB / 32];
-  __shared__ int s_idx[kNmsTPB / 32];
+  float* work = scratch + (size_t)base * 6;     // [N,5] the rows by position (score -1: removed in this round)
+  int* slot = reinterpret_cast<int*>(work + (size_t)N * 5);   // [N] compaction: hole positions up, movers down
+  __shared__ float s_val[kNmsWarps];
+  __shared__ int s_pos[kNmsWarps];
+  __shared__ int s_cnt[kNmsWarps];
   __shared__ float s_t[5];
-  __shared__ int s_stop;
-  for (int i = threadIdx.x; i < N * 5; i += blockDim.x) work[i] = d[i];
+  __shared__ int s_moves, s_stop;
+  for (int i = tid; i < N * 5; i += kNmsTPB) work[i] = d[i];
   __syncthreads();
-  int taken = 0;
-  for (;;) {
-    // ---- argmax over the remaining rows (scores are >= threshold > 0 or original; removed rows carry -1)
+  int live = N;
+  for (int i = 0; i < live; ++i) {
+    // ---- take: the highest score at positions [i, live), the lowest position on ties
     float best = -1.f;
-    int bi = -1;
-    for (int j = threadIdx.x; j < N; j += blockDim.x) {
-      const float s = work[5 * j + 4];
-      if (s > best) { best = s; bi = j; }          // strict >: the lowest row index wins a tie within a thread
+    int bq = INT_MAX;
+    for (int q = i + tid; q < live; q += kNmsTPB) {
+      const float s = work[5 * q + 4];
+      if (s > best) { best = s; bq = q; }          // strict >: the lowest position wins a tie within a thread
     }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
       const float ob = __shfl_xor_sync(0xffffffffu, best, off);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-      if (ob > best || (ob == best && oi >= 0 && (bi < 0 || oi < bi))) { best = ob; bi = oi; }
+      const int oq = __shfl_xor_sync(0xffffffffu, bq, off);
+      if (ob > best || (ob == best && oq < bq)) { best = ob; bq = oq; }
     }
-    if ((threadIdx.x & 31) == 0) { s_val[threadIdx.x >> 5] = best; s_idx[threadIdx.x >> 5] = bi; }
+    if (lane == 0) { s_val[warp] = best; s_pos[warp] = bq; }
     __syncthreads();
-    if (threadIdx.x == 0) {
+    if (tid == 0) {
       float b = s_val[0];
-      int k = s_idx[0];
-      for (int w = 1; w < kNmsTPB / 32; ++w)
-        if (s_val[w] > b || (s_val[w] == b && s_idx[w] >= 0 && (k < 0 || s_idx[w] < k))) { b = s_val[w]; k = s_idx[w]; }
-      s_stop = (k < 0 || b < 0.f) ? 1 : 0;
+      int k = s_pos[0];
+      for (int w = 1; w < kNmsWarps; ++w)
+        if (s_val[w] > b || (s_val[w] == b && s_pos[w] < k)) { b = s_val[w]; k = s_pos[w]; }
+      s_stop = k == INT_MAX;                       // only scores the contract rules out (NaN, <= -1) remain
       if (!s_stop) {
 #pragma unroll
-        for (int c = 0; c < 5; ++c) s_t[c] = work[5 * k + c];
-        work[5 * k + 4] = -1.f;                    // taken
-#pragma unroll
-        for (int c = 0; c < 5; ++c) d[5 * taken + c] = s_t[c];
+        for (int c = 0; c < 5; ++c) {
+          s_t[c] = work[5 * k + c];
+          work[5 * k + c] = work[5 * i + c];
+          work[5 * i + c] = s_t[c];
+        }
       }
     }
     __syncthreads();
-    if (s_stop) break;
-    ++taken;
+    if (s_stop) {
+      live = i;
+      break;
+    }
     const float tx1 = s_t[0], ty1 = s_t[1], tx2 = s_t[2], ty2 = s_t[3];
-    // ---- decay / remove the others
-    for (int j = threadIdx.x; j < N; j += blockDim.x) {
-      const float s = work[5 * j + 4];
-      if (s < 0.f) continue;
-      const float x1 = work[5 * j], y1 = work[5 * j + 1], x2 = work[5 * j + 2], y2 = work[5 * j + 3];
+    // ---- decay / remove the rows at positions (i, live)
+    int removed = 0;
+    for (int q = i + 1 + tid; q < live; q += kNmsTPB) {
+      const float s = work[5 * q + 4];
+      const float x1 = work[5 * q], y1 = work[5 * q + 1], x2 = work[5 * q + 2], y2 = work[5 * q + 3];
       const float area = (float)(((double)(x2 - x1) + 1.0) * ((double)(y2 - y1) + 1.0));
       const float iw = (float)((double)(fminf(tx2, x2) - fmaxf(tx1, x1)) + 1.0);
       if (iw > 0) {
@@ -87,13 +98,54 @@ __global__ void __launch_bounds__(kNmsTPB) soft_nms_batched_kernel(float* __rest
           else if (method == 2) weight = (float)exp((double)(-(ov * ov) / sigma));
           else weight = ov > Nt ? 0.f : 1.f;
           const float ns = weight * s;
-          work[5 * j + 4] = ns < threshold ? -1.f : ns;
+          removed |= ns < threshold;
+          work[5 * q + 4] = ns < threshold ? -1.f : ns;
         }
       }
     }
+    if (!__syncthreads_or(removed)) continue;
+    // ---- compaction in the reference's swap-with-last order.  Thread t owns the contiguous positions [q0, q1) of
+    // (i, live); a block-wide scan of the survivor counts gives each position its survivor rank.
+    const int lo = i + 1, per = (live - lo + kNmsTPB - 1) / kNmsTPB;
+    const int q0 = min(live, lo + tid * per), q1 = min(live, q0 + per);
+    int mine = 0;
+    for (int q = q0; q < q1; ++q) mine += work[5 * q + 4] >= 0.f;
+    int incl = mine;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += v;
+    }
+    if (lane == 31) s_cnt[warp] = incl;
+    __syncthreads();
+    int before = incl - mine, M = 0;                // survivors before q0; survivors in all of (i, live)
+#pragma unroll
+    for (int w = 0; w < kNmsWarps; ++w) {
+      before += w < warp ? s_cnt[w] : 0;
+      M += s_cnt[w];
+    }
+    const int keep_end = lo + M;
+    // hole h (counting up below keep_end) -> slot[h]; survivor g at >= keep_end (counting down) -> slot[N - 1 - g].
+    // There are as many of one as of the other, at most (live - lo) / 2 each, so the two ends never meet.
+    for (int q = q0, r = before; q < q1; ++q) {
+      const bool alive = work[5 * q + 4] >= 0.f;
+      if (q == keep_end) s_moves = M - r;         // the survivors from here on fill the holes
+      if (q < keep_end && !alive) slot[q - lo - r] = q;
+      if (q >= keep_end && alive) slot[N - 1 - (M - 1 - r)] = q;
+      r += alive;
+    }
+    __syncthreads();
+    // the movers' positions are >= keep_end, the holes' below it: no row is read here after it is written
+    for (int h = tid; h < s_moves; h += kNmsTPB) {
+      const int to = slot[h], from = slot[N - 1 - h];
+#pragma unroll
+      for (int c = 0; c < 5; ++c) work[5 * to + c] = work[5 * from + c];
+    }
+    live = keep_end;
     __syncthreads();
   }
-  if (threadIdx.x == 0) out_counts[p] = taken;
+  for (int j = tid; j < live * 5; j += kNmsTPB) d[j] = work[j];
+  if (tid == 0) out_counts[p] = live;
 }
 
 // nmsp (lib/nms/nms.py:48-80, threshold 0.7) for one image per CTA: the proposal NMS that imdb.load_rpn_data runs on
@@ -194,8 +246,9 @@ extern "C" {
 
 // dets: [total, 5] (x1, y1, x2, y2, score) rows of all problems back to back, problem p = rows [offsets[p],
 // offsets[p+1]); rewritten in place: the first out_counts[p] rows of each segment are the surviving detections in the
-// order cpu_soft_nms returns them.  offsets: device int32 [P+1]; scratch: device float [total*5].  Scores must be >= 0.
-// method 1 = linear, 2 = Gaussian (the reference's TEST default), 3 = hard NMS.
+// order cpu_soft_nms returns them, exact score ties included.  offsets: device int32 [P+1]; scratch: device, 24 bytes
+// per row (total * 6 floats).  Scores must be >= 0.  method 1 = linear, 2 = Gaussian (the reference's TEST default),
+// 3 = hard NMS.
 int sniper_soft_nms_batched(float* dets, const int* offsets, int P, float sigma, float Nt, float threshold,
                             unsigned method, int* out_counts, float* scratch, void* stream) {
   if (P <= 0) return 0;

@@ -786,13 +786,13 @@ def train_metric_accum(rpn_prob, rpn_label, A, cls_prob, cls_label, counts, loss
 def soft_nms_batched(dets, offsets, *, sigma=0.55, Nt=0.3, threshold=0.001, method=2):
     """cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110) on every segment dets[offsets[p]:offsets[p+1]] ([.,5] rows x1,y1,x2,y2,score)
     at once.  Returns (dets_out, counts): the first counts[p] rows of segment p are its surviving detections in the
-    reference's output order; `dets` itself is not modified."""
+    reference's output order, exact score ties included; `dets` itself is not modified."""
     assert dets.is_cuda and dets.dtype == torch.float32 and dets.dim() == 2 and dets.shape[1] == 5 and dets.is_contiguous()
     assert offsets.dtype == torch.int32 and offsets.is_cuda
     P = offsets.numel() - 1
     out = dets.clone()
     counts = torch.zeros(max(P, 1), dtype=torch.int32, device=dets.device)
-    scratch = torch.empty_like(dets)
+    scratch = torch.empty((dets.shape[0], 6), dtype=torch.float32, device=dets.device)     # rows + compaction slots
     check(lib().sniper_soft_nms_batched(_ptr(out), _ptr(offsets), P, float(sigma), float(Nt), float(threshold), int(method),
                                         _ptr(counts), _ptr(scratch), _stream()))
     return out, counts[:P]

@@ -59,7 +59,7 @@ DOC = {
     "sniper_anchor_target": "RPN anchor matching of anchor_worker.worker (lib/data_utils/data_workers.py:164-371) on device.",
     "sniper_focus_label": "FocusPixel labels of anchor_worker.worker's gen_mask (lib/data_utils/data_workers.py:165-192, TRAIN.AUTO_FOCUS) on device: the AutoFocus training label scale_label [B, Hf*Wf].",
     "sniper_focus_acc": "AutoFocusAccMetric (lib/train_utils/metric.py:50-72) on device: argmax hits and non-ignored pixels of the FocusPixel softmax, accumulated as exact float counts.",
-    "sniper_soft_nms_batched":"cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110; Gaussian / linear / hard) for every (image, class) problem of an inference scale in ONE launch: replaces the Pool(32) of nms_worker processes in Tester.aggregate (lib/inference.py:152-200).",
+    "sniper_soft_nms_batched":"cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110; Gaussian / linear / hard) for every (image, class) problem of an inference scale in ONE launch: replaces the Pool(32) of nms_worker processes in Tester.aggregate (lib/inference.py:152-200). Same rows in the same order as the reference, exact score ties included (its row swaps are replayed); scratch: 24 bytes per row.",
     "sniper_proposal_nms_batched": "nmsp (lib/nms/nms.py:48-80, IoU threshold 0.7) of imdb.load_rpn_data (lib/dataset/imdb.py:81-118) for many images in ONE launch, one CTA per image: replaces the Pool(32) of host nmsp calls over the extracted RPN proposals. Keeps nmsp's float32 arithmetic and order; exact score ties go to the higher row.",
     "sniper_detect_post_workspace_bytes": "Scratch bytes for sniper_detect_post.",
     "sniper_detect_post": "Tester.detect's box decoding (lib/inference.py:100-139; nonlinear_pred lib/bbox/bbox_transform.py:93-133, clip_boxes, division by the scale), the score threshold and chip-border pruning of Tester.get_detections (lib/inference.py:232-351, check_valid :235-258) and the valid-range filter of Tester.aggregate (lib/inference.py:152-230, filter :176-186) for one batch of chips in ONE cooperative launch: surviving (x1, y1, x2, y2, score) rows appended to a caller-owned run buffer at a device-side cursor in (chip, roi, class) order, each with a 64-bit (image, class, scale, chip, roi) order key.  float64 decode, float32 rows rounded where the host path rounds them (no FMA).",
