@@ -22,6 +22,7 @@ from decimal import ROUND_HALF_UP, Decimal
 import numpy as np
 import torch
 
+from . import recall
 from .cocoeval import COCO, COCOeval
 
 
@@ -140,6 +141,12 @@ class coco(object):
                 'max_classes': overlaps.argmax(axis=1),
                 'max_overlaps': overlaps.max(axis=1),
                 'flipped': False}
+
+    def evaluate_recall(self, roidb, candidate_boxes=None, thresholds=None):
+        """Proposal recall per GT area range of the first num_images entries of roidb (recall.evaluate_recall): the
+        reference's info string, printed and returned."""
+        return recall.evaluate_recall(roidb, candidate_boxes, thresholds, num_images=self.num_images,
+                                      device=self.device)
 
     def evaluate_detections(self, detections):
         """Writes the results json and, for a non-test image set, evaluates it; returns COCOeval.stats (None for a test

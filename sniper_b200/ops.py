@@ -1061,3 +1061,106 @@ def voc_accumulate(flags, det_off, npos, use_07_metric, thresholds_07=None):
                                       det_off.ctypes.data, C, T, int(bool(use_07_metric)), t07.ctypes.data, t07.size,
                                       _ptr(rec), _ptr(prec), _ptr(ap), _ptr(terms), _stream()))
     return rec, prec, ap
+
+
+RECALL_RANGES = 7
+_RECALL_DTYPES = {np.dtype(np.uint16): 0, np.dtype(np.float32): 1, np.dtype(np.float64): 2}
+
+
+def proposal_recall(prop_box, prop_off, gt_box, gt_off, gt_range, thresholds, device="cuda",
+                    max_workspace_bytes=1 << 30):
+    """The matching and the statistics of IMDB.evaluate_recall (lib/dataset/imdb.py:291-397) on the device.
+
+    prop_box: host [N, 4] uint16, float32 or float64, every image's proposals as stored (image i at
+    prop_off[i]:prop_off[i+1]); gt_box: host [G, 4], the GTs the reference keeps, widened to float64 (image i at
+    gt_off[i]:gt_off[i+1]); gt_range: host [G] uint8, bit r set when the GT's area (in its own dtype) lies in area range
+    r (0 = all, 1 .. 6 = 0-25 .. 300-inf); thresholds: host float64 [T].  Pairs whose IoU matrix does not fit in shared
+    memory use a device workspace, run in launches of at most `max_workspace_bytes` each (a single larger pair still
+    runs).  Returns a dict of host arrays at full precision: recalls [7, T], ar [7], num_pos [7], gt_overlaps (7 sorted
+    float64 arrays), area_counts [6] (proposals per range 1 .. 6), area_fraction [6] and avg_proposals."""
+    prop_off, gt_off = _off(prop_off), _off(gt_off)
+    I = prop_off.size - 1
+    if gt_off.size != I + 1:
+        raise ValueError("proposal_recall: prop_off and gt_off must have one entry per image plus one (%d, %d)"
+                         % (prop_off.size, gt_off.size))
+    prop_box, gt_box = np.asarray(prop_box), np.asarray(gt_box)
+    if prop_box.dtype not in _RECALL_DTYPES:
+        raise ValueError("proposal_recall: proposals must be uint16, float32 or float64, not %s" % prop_box.dtype)
+    N, G = int(prop_off[-1]), int(gt_off[-1])
+    if prop_box.shape != (N, 4) or gt_box.shape != (G, 4):
+        raise ValueError("proposal_recall: prop_box must be [N, 4] and gt_box [G, 4] (N = %d, G = %d), not %s and %s"
+                         % (N, G, prop_box.shape, gt_box.shape))
+    if gt_box.dtype != np.float64:
+        raise ValueError("proposal_recall: gt_box must be float64, not %s" % gt_box.dtype)
+    if not (np.isfinite(prop_box).all() and np.isfinite(gt_box).all()):
+        raise ValueError("proposal_recall: box coordinates must be finite")
+    gt_range = np.ascontiguousarray(gt_range, dtype=np.uint8).reshape(-1)
+    if gt_range.size != G:
+        raise ValueError("proposal_recall: gt_range must hold one mask per GT (%d), not %d" % (G, gt_range.size))
+    thr = np.asarray(thresholds)
+    if thr.ndim != 1 or thr.dtype != np.float64:
+        raise ValueError("proposal_recall: thresholds must be a 1-D float64 array")
+    thr = np.ascontiguousarray(thr)
+    T = thr.size
+    prop_box, gt_box = np.ascontiguousarray(prop_box), np.ascontiguousarray(gt_box)
+    L = lib()
+    P = RECALL_RANGES * I
+    ws_off = np.zeros(P + 1, np.int64)
+    check(L.sniper_proposal_recall_workspace_bytes(prop_off.ctypes.data, gt_off.ctypes.data, gt_range.ctypes.data, I,
+                                                   ws_off.ctypes.data))
+    # per (range, image): the GTs in range, and what the image adds to gt_overlaps (nothing without proposals)
+    bits = ((gt_range[:, None] >> np.arange(RECALL_RANGES, dtype=np.uint8)) & 1).astype(np.int64)
+    cs = np.vstack([np.zeros((1, RECALL_RANGES), np.int64), np.cumsum(bits, axis=0)])
+    m = (cs[gt_off[1:]] - cs[gt_off[:-1]]).T                              # [7, I]
+    contrib = np.where(np.diff(prop_off)[None, :] > 0, m, 0)
+    out_off = np.zeros(P + 1, np.int64)
+    np.cumsum(contrib.reshape(-1), out=out_off[1:])
+    num_pos = m.sum(axis=1).astype(np.int64)
+    range_off = np.ascontiguousarray(out_off[::I] if I else np.zeros(RECALL_RANGES + 1, np.int64))
+
+    dev = torch.device(device)
+    up = lambda a: torch.from_numpy(a).to(dev)  # noqa: E731
+    d_prop = up(prop_box.view(np.int16) if prop_box.dtype == np.uint16 else prop_box)
+    d_gt, d_range = up(gt_box), up(gt_range)
+    d_poff, d_goff, d_out_off, d_ws_off = up(prop_off), up(gt_off), up(out_off), up(ws_off)
+    overlaps = torch.empty(max(int(out_off[-1]), 1), dtype=torch.float64, device=dev)
+    status = torch.zeros(max(P, 1), dtype=torch.uint8, device=dev)
+    chunks, b = [], 0
+    while b < P:
+        e = int(np.searchsorted(ws_off, ws_off[b] + max_workspace_bytes, side="right")) - 1
+        e = min(max(e, b + 1), P)
+        chunks.append((b, e))
+        b = e
+    ws_need = max([int(ws_off[e] - ws_off[b]) for b, e in chunks] + [0])
+    ws = torch.empty(ws_need, dtype=torch.uint8, device=dev) if ws_need else None
+    dt = _RECALL_DTYPES[prop_box.dtype]
+    with torch.cuda.device(dev):
+        st = _stream()
+        for b, e in chunks:
+            check(L.sniper_proposal_recall_match(_ptr(d_prop), dt, _ptr(d_poff), _ptr(d_gt), _ptr(d_range),
+                                                 _ptr(d_goff), _ptr(d_out_off), _ptr(d_ws_off), prop_off.ctypes.data,
+                                                 gt_off.ctypes.data, gt_range.ctypes.data, ws_off.ctypes.data, I, b, e,
+                                                 _ptr(ws), _ptr(overlaps), _ptr(status), st))
+        counts = torch.empty(RECALL_RANGES * T + 6, dtype=torch.int64, device=dev)
+        done = torch.empty(1, dtype=torch.int32, device=dev)
+        recalls = torch.empty(max(RECALL_RANGES * T, 1), dtype=torch.float64, device=dev)
+        ar = torch.empty(RECALL_RANGES, dtype=torch.float64, device=dev)
+        hist = torch.empty(7, dtype=torch.float64, device=dev)
+        d_thr = up(thr) if T else None
+        check(L.sniper_proposal_recall_accumulate(_ptr(overlaps), range_off.ctypes.data, num_pos.ctypes.data,
+                                                  _ptr(d_thr), T, _ptr(d_prop), dt, N, I, _ptr(counts), _ptr(done),
+                                                  _ptr(recalls), _ptr(ar), _ptr(hist), st))
+    bad = np.flatnonzero(status.cpu().numpy()[:P])
+    if bad.size:
+        p = int(bad[0])
+        why = {1: "its best overlap is negative", 2: "an IoU has a zero union"}[int(status[p])]
+        raise ValueError("proposal_recall: image %d, area range %d: %s (the reference asserts / divides by zero)"
+                         % (p % I, p // I, why))
+    ov = overlaps.cpu().numpy()
+    cnt = counts.cpu().numpy()
+    h = hist.cpu().numpy()
+    return dict(recalls=recalls.cpu().numpy()[:RECALL_RANGES * T].reshape(RECALL_RANGES, T), ar=ar.cpu().numpy(),
+                num_pos=num_pos, gt_overlaps=[np.sort(ov[range_off[r]:range_off[r + 1]])
+                                              for r in range(RECALL_RANGES)],
+                area_counts=cnt[RECALL_RANGES * T:].astype(np.int64), area_fraction=h[:6],
+                avg_proposals=float(h[6]))

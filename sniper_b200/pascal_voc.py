@@ -24,7 +24,7 @@ import xml.etree.ElementTree as ET
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, recall
 
 CLASSES = ('__background__',  # always index 0
            'aeroplane', 'bicycle', 'bird', 'boat', 'bottle', 'bus', 'car', 'cat', 'chair', 'cow', 'diningtable', 'dog',
@@ -274,6 +274,12 @@ class PascalVOC(object):
                 continue
             with open(self.get_result_file_template().format(cls), 'wt') as f:
                 f.write(self.results_text(all_boxes, cls_ind))
+
+    def evaluate_recall(self, roidb, candidate_boxes=None, thresholds=None):
+        """Proposal recall per GT area range of the first num_images entries of roidb (recall.evaluate_recall): the
+        reference's info string, printed and returned."""
+        return recall.evaluate_recall(roidb, candidate_boxes, thresholds, num_images=self.num_images,
+                                      device=self.device)
 
     def evaluate_detections(self, detections):
         """Writes the comp4 files and evaluates them (pascal_voc.py:246-265); returns do_python_eval's info string.

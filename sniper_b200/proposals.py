@@ -24,7 +24,7 @@ import pickle
 import numpy as np
 import torch
 
-from . import host, ops
+from . import host, ops, recall
 
 NMS_CHUNK = 4096          # images per device launch
 
@@ -118,6 +118,12 @@ class IMDB(object):
                        'proposal_scores': scores}
             roidb.append(roi_rec)
         return roidb
+
+    def evaluate_recall(self, roidb, candidate_boxes=None, thresholds=None):
+        """Proposal recall per GT area range of every entry of roidb, which gives the image count this class lacks
+        (recall.evaluate_recall): the reference's info string, printed and returned."""
+        return recall.evaluate_recall(roidb, candidate_boxes, thresholds, num_images=len(roidb),
+                                      device=self.device)
 
     @staticmethod
     def merge_roidbs(a, b):

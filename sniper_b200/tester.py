@@ -453,12 +453,15 @@ def proposal_file_name(config):
 
 
 def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0",
-                                     image_loader=None):
+                                     image_loader=None, imdb=None):
     """The CONCURRENT_JOBS == 1 path of imdb_proposal_extraction_wrapper (:559-610): RPN proposals of every image at every
     scale of TEST.SCALES (`net.forward_rpn`), each image's rows stacked in scale order, pickled as a list of float32
     [n, 5] arrays to save_path/proposal_file_name(config) (protocol 2, readable by the reference's Python 2).  Returns
     (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds.  image_loader(path)
-    decodes the entries without 'image_data' (e.g. host.imread)."""
+    decodes the entries without 'image_data' (e.g. host.imread).  With an imdb (`coco.coco`, `pascal_voc.PascalVOC`
+    or `proposals.IMDB`), the recall of the extracted proposals follows: imdb.evaluate_recall(roidb, candidate_boxes=
+    [p[:, :4] for p in proposals]) against the GT fields of `roidb` (boxes / gt_classes / gt_overlaps), whose string
+    goes to stats['recall'] and its seconds to stats['recall_s']."""
     T = config.TEST
     proposals, stats = [], dict(scales=[])
     nb = batch_images or list(T.BATCH_IMAGES)
@@ -473,4 +476,8 @@ def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images
     os.makedirs(save_path, exist_ok=True)
     with open(os.path.join(save_path, proposal_file_name(config)), 'wb') as f:
         pickle.dump(final, f, protocol=2)
+    if imdb is not None:
+        t0 = time.time()
+        stats['recall'] = imdb.evaluate_recall(roidb, candidate_boxes=[p[:, :4] for p in final])
+        stats['recall_s'] = time.time() - t0
     return final, stats

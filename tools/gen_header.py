@@ -75,6 +75,9 @@ DOC = {
     "sniper_coco_accumulate": "COCOeval.accumulate (lib/dataset/pycocotools/cocoeval.py:274-374): precision[T,R,K,A,M] and recall[T,K,A,M] float64, one block per (category, area, maxDet, threshold), from sniper_coco_match's flags and one stable (category, descending score) order of the detections (cat_order) with their in-image ranks (dt_rank).  Byte-equal to the reference, -1 where it leaves -1.",
     "sniper_voc_match": "The matching loop of voc_eval (lib/dataset/pascal_voc_eval.py:137-171) for every (class, image) pair x overlap threshold in ONE launch, the pair's detections in the host's np.argsort(-confidence) order (:127-131): overlaps with +1 pixel extents, ovmax / jmax as np.max / np.argmax (a NaN wins, first maximum), the strict `ovmax > ovthresh`, difficult GTs neither tp nor fp, a second hit on a taken GT an fp.  flags[T,N] uint8: 1 tp, 2 fp, 0 neither; taken[T,G] is the reference's det scratch.  Bit-exact (no FMA).",
     "sniper_voc_accumulate": "pascal_voc_eval.py:173-179 and voc_ap (:39-70) for every class x threshold, one block each: integer tp / fp scans, rec = tp / float(npos), prec = tp / max(tp + fp, eps), then the 11-point AP (host recall thresholds, ap += p / 11. in order) or the area AP (mpre envelope, terms where mrec changes summed in numpy's pairwise order; terms is [T, N + C] scratch).  rec / prec [T,N] and ap [T,C] float64, byte-equal to the reference's.",
+    "sniper_proposal_recall_workspace_bytes": "Host-only: per (area range, image) pair p = r * num_images + i, the byte offset of its IoU matrix in the workspace of sniper_proposal_recall_match (pair_ws_off_host[7 * num_images + 1]; pairs whose matrix fits in shared memory take none).  The workspace of pairs [b, e) is pair_ws_off[e] - pair_ws_off[b] bytes; the library never allocates it.",
+    "sniper_proposal_recall_match": "The greedy matching of IMDB.evaluate_recall (lib/dataset/imdb.py:329-374) for pairs [pair_begin, pair_end) of (area range, image) in ONE launch, one block per pair: IoUs as bbox_overlaps_cython (lib/bbox/bbox.pyx:17-57) in float64 from uint16 / float32 / float64 proposals (prop_dtype 0 / 1 / 2) and float64 GTs; each round the best unused column maximum (argmax ties to the lower row, then the lower column), its row and column retired.  Writes each pair's round overlaps then zeros at gt_overlaps + pair_out_off[p]; status[p] = 1 where the reference asserts (best overlap < 0), 2 where bbox_overlaps_cython divides by zero.  Bit-exact (no FMA).",
+    "sniper_proposal_recall_accumulate": "The statistics of IMDB.evaluate_recall (lib/dataset/imdb.py:307-328, 376-394) in ONE launch: counts[r * T + t] of gt_overlaps >= thresholds[t] per area range, then counts[7 * T + k] the proposals whose area (in their dtype) lies in range k + 1; recalls[r * T + t] = count / float(num_pos[r]), ar[r] = recalls.mean() in numpy's pairwise order, hist[k] = area_count / total_counts and hist[6] = total_counts / num_images.  counts / done are zeroed on the stream first.",
     "sniper_train_metric_workspace_bytes": "Scratch bytes for sniper_train_metric_accum (zero-filled once by the caller; the kernel leaves it reusable).",
     "sniper_train_metric_accum": "The training metrics of lib/train_utils/metric.py:50-95, 104-300 (RPNAcc, RPNLogLoss, RPNL1Loss, RCNNAcc, RCNNLogLoss, RCNNL1LossCRCNN, AutoFocusAcc, AutoFocusLogLoss) for one step in ONE launch, added into a caller-owned accumulator (int64 num_inst[8] | int64 hits[8] | float64 sum[8]): replaces their per-step asnumpy() (:109-125).  Argmax ties to the first maximum, p + 1e-14 in float32, log and sums in float64, block partials summed in block order (byte-identical run to run).  num_inst from the step's count_valid results, the L1 sums from its loss buffer.",
     "sniper_nms_gpu":"Batched hard NMS on device for per-scale inference NMS (lib/nms/nms_kernel.cu:34-144 replacement).",
