@@ -87,6 +87,8 @@ SIGNATURES = {
     "sniper_proposal_recall_workspace_bytes": ("i", "ppp" "i" "p"),
     "sniper_proposal_recall_match": ("i", "pip" "ppppp" "pppp" "iii" "pppp"),
     "sniper_proposal_recall_accumulate": ("i", "pppp" "i" "pi" "li" "ppppp" "p"),
+    "sniper_focus_chips_workspace_bytes": ("i", "pip"),
+    "sniper_focus_chips": ("i", "pppp" "i" "ifi" "p" "i" "pp" "p"),
     "sniper_train_metric_workspace_bytes": ("z", ""),
     "sniper_train_metric_accum": ("i", "pipiiii" "pipii" "pipii" "ppppp"),
 }
@@ -99,7 +101,7 @@ KERNELS_PER_CALL = {
     "sniper_set_stream_workspace": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
     "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
     "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0,
-    "sniper_proposal_recall_workspace_bytes": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
+    "sniper_proposal_recall_workspace_bytes": 0, "sniper_focus_chips_workspace_bytes": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,
     "sniper_depthwise3x3_wgrad": 2,
     # the operand copy kernel + the wgmma kernel of tf32 3 x 3 layers; other calls launch only the latter (counted as 2

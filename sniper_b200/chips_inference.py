@@ -14,11 +14,17 @@ restated here from the OpenCV documentation):
 Contours are listed last-found-first (raster scan of the start pixel, the order `RETR_LIST` yields).  Everything else --
 the integer arithmetic of the merge loop (Python 2 `/` on ints = floor division), the iteration until the chip count
 stops changing, the rescaling -- follows the reference line by line.
+
+The device detection backend leaves its FocusPixel maps on the GPU (`DeviceFocusMaps`); `add_chips` given those runs
+`gmask` for every map of the scale in one `ops.focus_chips` launch (csrc/focus_chips.cu), byte-equal to the host code
+here, which stays the specification the kernel is tested against.
 """
 import math
 
 import numpy as np
 from scipy import ndimage
+
+from . import ops
 
 _S8 = np.ones((3, 3), dtype=bool)
 _S4 = np.array([[0, 1, 0], [1, 1, 1], [0, 1, 0]], dtype=bool)
@@ -138,7 +144,10 @@ def image_scale(width, height, target):
 def add_chips(roidb, maps, scale_id, cfg):
     """Replaces every image's `inference_crops` by the FocusChips found at scale `scale_id` (to be processed at scale
     scale_id + 1).  maps[i][j] = (anything, FocusPixel map of crop j of image i).  Returns [chip_area, total_area] in
-    megapixels at the next scale (chips_inference.py:91-173)."""
+    megapixels at the next scale (chips_inference.py:91-173).  `maps` may be a `DeviceFocusMaps`: the FocusChips then
+    come from the device, with the same values, order and return value."""
+    if isinstance(maps, DeviceFocusMaps):
+        return _add_chips_device(roidb, maps, scale_id, cfg)
     total_area = 0
     chip_area = 0
     hp = cfg.TEST.CHIP_HYPERPARAMS[scale_id]
@@ -165,6 +174,102 @@ def add_chips(roidb, maps, scale_id, cfg):
                 chip_area = chip_area + tarea / (1000. * 1000.)
             cur_chips += chips
         roidb[i]['inference_crops'] = np.array(cur_chips)
+    return [chip_area, total_area]
+
+
+class DeviceFocusMaps(object):
+    """The FocusPixel maps of one test scale as the network left them on the device: per batch the `focus_map` output
+    [B, Hc, Wc] (kept alive, not copied) and each row's map extents, ceil(resized h / stride) x ceil(resized w / stride)
+    as `Tester._chip_maps` cuts them.  maps[i][j] is (None, host float32 copy of crop j's map of image i), made on
+    access, or [] when no batch carried that crop, like the host backend's all_maps; a later batch replaces the map an
+    earlier one gave a crop (the iterator repeats crops to fill its batches)."""
+
+    def __init__(self, n_chips, feat_stride):
+        self.stride = float(feat_stride)
+        self.tensors, self.extents = [], []
+        self.where = [[None] * int(n) for n in n_chips]
+
+    def add(self, fm, im_info, im_ids, chip_ids):
+        """One batch: fm [B, Hc, Wc] float32 on the device, im_info host float32 [B, 3] (resized h, resized w, scale);
+        row b is crop chip_ids[b] of image im_ids[b]."""
+        info = np.asarray(im_info, dtype=np.float32).reshape(-1, 3)
+        k = len(self.tensors)
+        self.tensors.append(fm)
+        self.extents.append(np.stack([np.ceil(info[:, 0] / self.stride), np.ceil(info[:, 1] / self.stride)],
+                                     1).astype(np.int64))
+        for b, (i, j) in enumerate(zip(im_ids, chip_ids)):
+            self.where[int(i)][int(j)] = (k, b)
+
+    def __len__(self):
+        return len(self.where)
+
+    def __getitem__(self, i):
+        return _ImageFocusMaps(self, i)
+
+    def focus_table(self, roidb, scale):
+        """The `ops.focus_chips` inputs of every (image, crop) in roidb order: (index int64 [n, 6] = batch, row, H, W,
+        iw, ih; geometry float64 [n, 5] = im_width, im_height, cscale, crop x1, crop y1), each value from add_chips' /
+        gmask's own expression (cscale = image_scale at `scale`, im_width = crop width * cscale, iw = ceil(im_width /
+        16))."""
+        index, geometry = [np.zeros((0, 6), np.int64)], [np.zeros((0, 5))]
+        for i, r in enumerate(roidb):
+            crops = np.asarray(r['inference_crops'])
+            if len(crops) != len(self.where[i]):
+                raise ValueError("DeviceFocusMaps: image %d has %d crops and %d maps" % (i, len(crops), len(self.where[i])))
+            if not len(crops):
+                continue
+            if any(w is None for w in self.where[i]):
+                raise ValueError("DeviceFocusMaps: crop %d of image %d has no map" % (self.where[i].index(None), i))
+            crops = crops.reshape(-1, 4)
+            cscale = image_scale(r['width'], r['height'], scale)
+            imw = np.asarray((crops[:, 2] - crops[:, 0]) * cscale, np.float64)
+            imh = np.asarray((crops[:, 3] - crops[:, 1]) * cscale, np.float64)
+            kb = np.array(self.where[i], np.int64)
+            hw = np.array([self.extents[k][b] for k, b in self.where[i]], np.int64)
+            index.append(np.column_stack([kb, hw, np.ceil(imw / 16), np.ceil(imh / 16)]).astype(np.int64))
+            geometry.append(np.column_stack([imw, imh, np.full(len(crops), cscale), crops[:, 0], crops[:, 1]])
+                            .astype(np.float64))
+        return np.concatenate(index), np.concatenate(geometry)
+
+
+class _ImageFocusMaps(object):
+    """maps[i] of a `DeviceFocusMaps`: one entry per crop of image i."""
+
+    def __init__(self, maps, i):
+        self._maps, self._where = maps, maps.where[i]
+
+    def __len__(self):
+        return len(self._where)
+
+    def __getitem__(self, j):
+        w = self._where[j]
+        if w is None:
+            return []
+        k, b = w
+        H, W = self._maps.extents[k][b]
+        return (None, np.ascontiguousarray(self._maps.tensors[k][b, :H, :W].cpu().numpy()))
+
+
+def _add_chips_device(roidb, maps, scale_id, cfg):
+    """add_chips for a `DeviceFocusMaps`: the FocusChips of every map from one `ops.focus_chips` launch, then the area
+    sums on the host with add_chips' expressions, in its order."""
+    hp = cfg.TEST.CHIP_HYPERPARAMS[scale_id]
+    index, geometry = maps.focus_table(roidb, cfg.TEST.SCALES[scale_id])
+    chips, off = ops.focus_chips(maps.tensors, index, geometry, d=hp[0], thresh=hp[1], ms=hp[2])
+    total_area = 0
+    chip_area = 0
+    m = 0
+    for i, r in enumerate(roidb):
+        im_width, im_height = r['width'], r['height']
+        tcscale = image_scale(im_width, im_height, cfg.TEST.SCALES[scale_id + 1])
+        total_area = total_area + (im_width * im_height * tcscale * tcscale) / (1000. * 1000.)
+        n = len(maps[i])
+        cur = chips[off[m]:off[m + n]]
+        m += n
+        for c in cur:
+            tarea = (c[2] - c[0]) * (c[3] - c[1]) * tcscale * tcscale
+            chip_area = chip_area + tarea / (1000. * 1000.)
+        roidb[i]['inference_crops'] = cur.copy() if len(cur) else np.array([])
     return [chip_area, total_area]
 
 

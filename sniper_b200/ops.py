@@ -1164,3 +1164,114 @@ def proposal_recall(prop_box, prop_off, gt_box, gt_off, gt_range, thresholds, de
                                               for r in range(RECALL_RANGES)],
                 area_counts=cnt[RECALL_RANGES * T:].astype(np.int64), area_fraction=h[:6],
                 avg_proposals=float(h[6]))
+
+
+# ---------------------------------------------------------------------------------------------
+# AutoFocus FocusChips (lib/chips/chips_inference.py:12-173)
+# ---------------------------------------------------------------------------------------------
+FOCUS_TABLE_COLS = 12
+
+
+def focus_threshold(thresh):
+    """The float32 t for which `v >= t` in float32 equals numpy's `float32 map >= thresh` for every float32 v: a Python
+    float or int compares in float32 (t = float32(thresh)); a numpy float64 compares in double, which for float32 values
+    is the comparison with the least float32 not below thresh."""
+    t = np.float32(thresh)
+    if np.result_type(np.float32, thresh) != np.float32 and float(t) < float(thresh):
+        t = np.nextafter(t, np.float32(np.inf))
+    return t
+
+
+def focus_chips_table(maps, index, geometry):
+    """The int64 [n, 12] table of `sniper_focus_chips` (validated): see `focus_chips` for maps / index / geometry."""
+    index = np.asarray(index)
+    geometry = np.asarray(geometry)
+    if index.ndim != 2 or index.shape[1] != 6 or index.dtype.kind not in "iu":
+        raise ValueError("focus_chips: index must be an integer [n, 6] array, not %s %s" % (index.dtype, index.shape))
+    n = index.shape[0]
+    if geometry.shape != (n, 5) or geometry.dtype != np.float64:
+        raise ValueError("focus_chips: geometry must be float64 [%d, 5], not %s %s" % (n, geometry.dtype, geometry.shape))
+    if not (np.isfinite(geometry).all() and (geometry[:, 2] > 0).all()):
+        raise ValueError("focus_chips: geometry must be finite with a positive cscale")
+    if not maps:
+        if n:
+            raise ValueError("focus_chips: %d maps refer to no tensor" % n)
+        return np.zeros((0, FOCUS_TABLE_COLS), np.int64)
+    dev = maps[0].device
+    for k, t in enumerate(maps):
+        if not (torch.is_tensor(t) and t.is_cuda and t.device == dev and t.dtype == torch.float32 and t.dim() == 3):
+            raise ValueError("focus_chips: maps[%d] must be a float32 [B, H, W] tensor on %s" % (k, dev))
+    index = index.astype(np.int64)
+    ti, row, H, W, iw, ih = index.T
+    if n and (ti.min() < 0 or ti.max() >= len(maps)):
+        raise ValueError("focus_chips: index names a tensor outside maps[0:%d]" % len(maps))
+    shape = np.array([t.shape for t in maps], np.int64).reshape(-1, 3)
+    stride = np.array([t.stride() for t in maps], np.int64).reshape(-1, 3)
+    base = np.array([t.data_ptr() for t in maps], np.int64)
+    if n and ((row < 0) | (row >= shape[ti, 0]) | (H < 0) | (H > shape[ti, 1]) | (W < 0) | (W > shape[ti, 2])).any():
+        raise ValueError("focus_chips: a map's row / H / W lies outside its tensor")
+    if n and ((iw < 0) | (ih < 0)).any():
+        raise ValueError("focus_chips: iw / ih must not be negative")
+    if n and ((base[ti] == 0) & (H * W > 0)).any():
+        raise ValueError("focus_chips: a map's tensor has a null address")
+    table = np.zeros((n, FOCUS_TABLE_COLS), np.int64)
+    table[:, 0] = base[ti] + row * stride[ti, 0] * 4
+    table[:, 1], table[:, 2] = stride[ti, 1], stride[ti, 2]
+    table[:, 3:7] = index[:, 2:6]
+    table[:, 7:12] = np.ascontiguousarray(geometry).view(np.int64)
+    return table
+
+
+def focus_chips(maps, index, geometry, *, d, thresh, ms, capacity=8):
+    """gmask (lib/chips/chips_inference.py:12-89) and the crop shift of add_chips (:158-162) for many FocusPixel maps in
+    one `sniper_focus_chips` launch, the maps read in place.
+
+    maps: device float32 tensors [B, Hc, Wc] (any strides: the `focus_map` view is fine); index: host int64 [n, 6] per map
+    (tensor, row, H, W, iw, ih): map m is maps[tensor][row, :H, :W] and iw / ih are gmask's ceil(im_width / 16) /
+    ceil(im_height / 16); geometry: host float64 [n, 5] per map (im_width, im_height, cscale, crop x1, crop y1).
+    d, thresh, ms: the scale's CHIP_HYPERPARAMS.  Returns (chips, offsets): host float64 [total, 4] and int64 [n + 1], map
+    m's FocusChips in image coordinates and gmask's order at chips[offsets[m]:offsets[m + 1]].  Waits for the launch; maps
+    with more than `capacity` chips run once more with room for all of them."""
+    if int(d) != d or d < 1 or int(ms) != ms or ms < 0:
+        raise ValueError("focus_chips: d (%r) must be an integer >= 1 and ms (%r) an integer >= 0" % (d, ms))
+    maps = list(maps)
+    table = focus_chips_table(maps, index, geometry)
+    n = table.shape[0]
+    if n == 0:
+        return np.zeros((0, 4)), np.zeros(1, np.int64)
+    dev = maps[0].device
+    H, W = table[:, 3], table[:, 4]
+    L = lib()
+    ws_off = np.zeros(n + 1, np.int64)
+    check(L.sniper_focus_chips_workspace_bytes(table.ctypes.data, n, ws_off.ctypes.data))
+    cap = max(int(capacity), 1)
+    up = lambda a: torch.from_numpy(a).to(dev)  # noqa: E731
+    with torch.cuda.device(dev):
+        d_table, d_ws_off = up(table), up(ws_off)
+        ws = torch.empty(int(ws_off[-1]), dtype=torch.uint8, device=dev) if ws_off[-1] else None
+        chips = torch.empty((max(n, 1), cap, 4), dtype=torch.float64, device=dev)
+        counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        check(L.sniper_focus_chips(_ptr(d_table), _ptr(d_ws_off), table.ctypes.data, ws_off.ctypes.data, n, int(d),
+                                   float(focus_threshold(thresh)), int(ms), _ptr(ws), cap, _ptr(chips), _ptr(counts),
+                                   _stream()))
+        cnt = counts.cpu().numpy()[:n].astype(np.int64)
+        got = chips.cpu().numpy()
+    bad = np.flatnonzero(cnt < 0)
+    if bad.size:
+        m = int(bad[0])
+        why = {-1: "the merge loop did not settle within H * W + 2 passes",
+               -2: "the table disagrees with its workspace offsets"}[int(cnt[m])]
+        raise _libmod.SniperError("focus_chips: map %d (%d x %d): %s" % (m, H[m], W[m], why))
+    off = np.zeros(n + 1, np.int64)
+    np.cumsum(cnt, out=off[1:])
+    out = np.empty((int(off[-1]), 4))
+    over = cnt > cap
+    m_i, k_i = np.nonzero((np.arange(cap)[None, :] < cnt[:, None]) & ~over[:, None])
+    out[off[m_i] + k_i] = got[m_i, k_i]
+    if over.any():
+        sel = np.flatnonzero(over)
+        more, more_off = focus_chips(maps, np.asarray(index)[sel], np.asarray(geometry)[sel], d=d, thresh=thresh, ms=ms,
+                                     capacity=int(cnt[sel].max()))
+        for q, m in enumerate(sel):
+            out[off[m]:off[m + 1]] = more[more_off[q]:more_off[q + 1]]
+    return out, off

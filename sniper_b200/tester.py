@@ -14,7 +14,9 @@ Host-side mirror of `lib/iterators/MNIteratorTestAutoFocus.py` (:13-141), `lib/i
                                                         the soft-NMS has run)
   per-(image, class) cpu_soft_nms in a Pool(32)         `inference.aggregate`, one path for both backends: ONE
                                                         `sniper_soft_nms_batched` launch for the whole run
-  FocusChips with OpenCV                                `chips_inference.add_chips`
+  FocusChips with OpenCV                                `chips_inference.add_chips`; with backend="device" the
+                                                        FocusPixel maps stay on the GPU and one `sniper_focus_chips`
+                                                        launch per scale finds the chips of all of them
 
 The proposal extraction of main_test.py with TEST.EXTRACT_PROPOSALS -- `MNIteratorTest`, `Tester.get_proposals` /
 `extract_proposals` and `imdb_proposal_extraction_wrapper` (lib/iterators/MNIteratorTest.py, lib/inference.py:76-98,
@@ -88,7 +90,7 @@ class _ImageCanvas(object):
         data = torch.empty(n, 3, SH, SW, device=dev)
         check(lib().sniper_chip_input_hw(self._pix.data_ptr(), tab.data_ptr(), self.means.data_ptr(), data.data_ptr(), n, SH,
                                          SW, torch.cuda.current_stream().cuda_stream))
-        return dict(data=data, im_info=torch.from_numpy(im_info).to(dev))
+        return dict(data=data, im_info=torch.from_numpy(im_info).to(dev), im_info_host=im_info)
 
 
 class DetectionNetwork(Protocol):
@@ -361,12 +363,13 @@ class Tester(object):
 
     def _get_detections_device(self, cls_thresh, do_pruning, autofocus, scale_index):
         """The batches of the scale with the detections kept on the device: `forward_inference`, then `ops.detect_post`
-        on its output tensors, fed by the batch's chip table.  Only the FocusPixel maps come to the host (FocusChips are
-        generated there), by non-blocking copies into pinned memory that are waited for once, after the last batch."""
+        on its output tensors, fed by the batch's chip table.  all_maps is a `chips_inference.DeviceFocusMaps`: each
+        batch's FocusPixel map tensor stays on the device (no map is copied to the host) for `add_chips` to run
+        `ops.focus_chips` on; maps[i][j] still gives a host copy."""
         want_map = bool(getattr(self.cfg.TEST, "AUTO_FOCUS", False)) and self.net.af is not None
         dets = inference.DeviceDetections(self.net.device)
-        all_maps = [[[] for _ in r['inference_crops']] for r in self.roidb]
-        seen, staged = set(), []
+        all_maps = chips_inference.DeviceFocusMaps([len(r['inference_crops']) for r in self.roidb], self.net.feat_stride)
+        seen = set()
         t0 = time.time()
         for batch in self.test_iter:
             out = self.net.forward_inference(batch['data'], batch['im_info'], autofocus=want_map)
@@ -375,18 +378,9 @@ class Tester(object):
                                          self.cfg.TEST.VALID_RANGES[scale_index], seen)
             dets.append(rois, cls_prob, deltas, batch['im_info'], table, cls_thresh=cls_thresh, scale=scale_index)
             if want_map and autofocus:
-                fm = torch.empty(out[4].shape, dtype=out[4].dtype, pin_memory=True)
-                info = torch.empty(batch['im_info'].shape, dtype=torch.float32, pin_memory=True)
-                fm.copy_(out[4], non_blocking=True)
-                info.copy_(batch['im_info'], non_blocking=True)
-                staged.append((fm, info, batch['im_ids'], batch['chip_ids']))
+                all_maps.add(out[4], batch['im_info_host'], batch['im_ids'], batch['chip_ids'])
         dets.finish()
         self.detect_time += time.time() - t0
-        t0 = time.time()
-        for fm, info, im_ids, chip_ids in staged:
-            for m, im_id, chip_id in zip(self._chip_maps(fm.numpy(), info.numpy()), im_ids, chip_ids):
-                all_maps[im_id][chip_id] = (None, m)
-        self.post_time += time.time() - t0
         return dets, all_maps
 
     def aggregate(self, scale_cls_dets, vis=False, cache_name='cache', vis_path=None, vis_name=None, pre_nms_db_divide=10,

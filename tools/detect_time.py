@@ -70,6 +70,8 @@ def pyramid(n_images, repeats):
                 row[k] = round(float(np.mean([x[k] for x in st])), 4)
             if 'detections_pre_nms' in st[0]:
                 row['detections_pre_nms'] = st[0]['detections_pre_nms']
+            if 'chip_gen_s' in st[0]:
+                row['chip_gen_s'] = round(float(np.mean([x['chip_gen_s'] for x in st])), 4)
             per_scale.append(row)
         agg = [r[1]['nms_s'] for r in runs[b]]
         out[b] = dict(images_per_s=round(n_images / secs.mean(), 3), images_per_s_min=round(n_images / secs.max(), 3),
@@ -80,10 +82,11 @@ def pyramid(n_images, repeats):
               "detections" % (b, out[b]['images_per_s'], out[b]['images_per_s_min'], out[b]['images_per_s_max'], repeats,
                               n_images, out[b]['aggregate_s'], final[b]), flush=True)
         for row in per_scale:
-            print("         scale %s: %d chips in %d batches, detect %.3f s, post %.3f s, total %.3f s%s"
+            print("         scale %s: %d chips in %d batches, detect %.3f s, post %.3f s, total %.3f s%s%s"
                   % (row['scale'], row['chips'], row['batches'], row['detect_s'], row['post_s'], row['total_s'],
                      ", %d rows pass the threshold and filters" % row['detections_pre_nms']
-                     if 'detections_pre_nms' in row else ""), flush=True)
+                     if 'detections_pre_nms' in row else "",
+                     ", FocusChips %.4f s" % row['chip_gen_s'] if 'chip_gen_s' in row else ""), flush=True)
     del net
     torch.cuda.empty_cache()
     return out, list(cfg.TEST.BATCH_IMAGES)

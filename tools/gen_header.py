@@ -78,6 +78,8 @@ DOC = {
     "sniper_proposal_recall_workspace_bytes": "Host-only: per (area range, image) pair p = r * num_images + i, the byte offset of its IoU matrix in the workspace of sniper_proposal_recall_match (pair_ws_off_host[7 * num_images + 1]; pairs whose matrix fits in shared memory take none).  The workspace of pairs [b, e) is pair_ws_off[e] - pair_ws_off[b] bytes; the library never allocates it.",
     "sniper_proposal_recall_match": "The greedy matching of IMDB.evaluate_recall (lib/dataset/imdb.py:329-374) for pairs [pair_begin, pair_end) of (area range, image) in ONE launch, one block per pair: IoUs as bbox_overlaps_cython (lib/bbox/bbox.pyx:17-57) in float64 from uint16 / float32 / float64 proposals (prop_dtype 0 / 1 / 2) and float64 GTs; each round the best unused column maximum (argmax ties to the lower row, then the lower column), its row and column retired.  Writes each pair's round overlaps then zeros at gt_overlaps + pair_out_off[p]; status[p] = 1 where the reference asserts (best overlap < 0), 2 where bbox_overlaps_cython divides by zero.  Bit-exact (no FMA).",
     "sniper_proposal_recall_accumulate": "The statistics of IMDB.evaluate_recall (lib/dataset/imdb.py:307-328, 376-394) in ONE launch: counts[r * T + t] of gt_overlaps >= thresholds[t] per area range, then counts[7 * T + k] the proposals whose area (in their dtype) lies in range k + 1; recalls[r * T + t] = count / float(num_pos[r]), ar[r] = recalls.mean() in numpy's pairwise order, hist[k] = area_count / total_counts and hist[6] = total_counts / num_images.  counts / done are zeroed on the stream first.",
+    "sniper_focus_chips_workspace_bytes": "Host-only: per FocusPixel map m of a sniper_focus_chips table, the byte offset of its scratch in the workspace (ws_off_host[n_maps + 1]; maps whose scratch fits in shared memory take none).  The library never allocates the workspace.",
+    "sniper_focus_chips": "gmask of the AutoFocus inference (lib/chips/chips_inference.py:12-89) with the crop shift of add_chips (:91-173) for every FocusPixel map of a test scale in ONE launch, one block per map: the float32 threshold (mask >= float32 thresh), cv2.dilate with a d x d window anchored at d // 2, the contours of cv2.findContours(RETR_LIST) (outer borders of 8-connected foreground components, hole borders of 4-connected background regions that touch no frame row or column, listed by start pixel descending), _place with Python floor division, the merge loop until the contour count repeats (more than H * W + 2 passes: counts[m] = -1), then the scaling to image coordinates in double.  table: int64 [n_maps, 12] per map = address of its cell (0, 0) (float32), row and column strides in elements, H, W, iw, ih, then the float64 bits of im_width, im_height, cscale and the crop origin x, y.  Writes counts[m] chips of map m as float64 (x1, y1, x2, y2) at chips + (m * cap + k) * 4, the first cap of them (the caller re-launches maps with more); counts[m] = -2 when the table disagrees with table_host / ws_off.  Bit-exact (no FMA).",
     "sniper_train_metric_workspace_bytes": "Scratch bytes for sniper_train_metric_accum (zero-filled once by the caller; the kernel leaves it reusable).",
     "sniper_train_metric_accum": "The training metrics of lib/train_utils/metric.py:50-95, 104-300 (RPNAcc, RPNLogLoss, RPNL1Loss, RCNNAcc, RCNNLogLoss, RCNNL1LossCRCNN, AutoFocusAcc, AutoFocusLogLoss) for one step in ONE launch, added into a caller-owned accumulator (int64 num_inst[8] | int64 hits[8] | float64 sum[8]): replaces their per-step asnumpy() (:109-125).  Argmax ties to the first maximum, p + 1e-14 in float32, log and sums in float64, block partials summed in block order (byte-identical run to run).  num_inst from the step's count_valid results, the L1 sums from its loss buffer.",
     "sniper_nms_gpu":"Batched hard NMS on device for per-scale inference NMS (lib/nms/nms_kernel.cu:34-144 replacement).",
