@@ -13,6 +13,7 @@
 #include <float.h>
 #include <limits.h>
 
+#include "block_reduce.cuh"
 #include "common.cuh"
 
 namespace {
@@ -153,41 +154,6 @@ __device__ __forceinline__ int upper_bound(const double* thr, int R, double v) {
   return lo;
 }
 
-__device__ __forceinline__ int3 add3(int3 a, int3 b) { return make_int3(a.x + b.x, a.y + b.y, a.z + b.z); }
-
-// inclusive block scan of (tp, fp, kept) counts; *total gets the block's sum
-__device__ int3 block_scan3(int3 v, int3* sh, int3* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int3 n = make_int3(__shfl_up_sync(~0u, v.x, o), __shfl_up_sync(~0u, v.y, o), __shfl_up_sync(~0u, v.z, o));
-    if (lane >= o) v = add3(v, n);
-  }
-  if (lane == 31) sh[warp] = v;
-  __syncthreads();
-  int3 before = make_int3(0, 0, 0), all = make_int3(0, 0, 0);
-  for (int w = 0; w < kAccWarps; ++w) {
-    if (w < warp) before = add3(before, sh[w]);
-    all = add3(all, sh[w]);
-  }
-  __syncthreads();
-  *total = all;
-  return add3(v, before);
-}
-
-// inclusive suffix max over the block (threads at and after this one)
-__device__ double block_suffix_max(double v, double* sh) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const double n = __shfl_down_sync(~0u, v, o);
-    if (lane + o < 32) v = fmax(v, n);
-  }
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  for (int w = warp + 1; w < kAccWarps; ++w) v = fmax(v, sh[w]);
-  __syncthreads();
-  return v;
-}
-
 // accumulate (cocoeval.py:274-374) for one (category, area range, maxDet, IoU threshold) per block.
 // cat_order lists the category's detections sorted by (descending score, concatenation order): the restriction of
 // that order to the detections of in-image rank < maxDet is the reference's mergesort of the maxDet-cut concatenation.
@@ -241,9 +207,9 @@ __global__ void __launch_bounds__(kAccTPB) coco_accumulate_kernel(
   };
   // pass 1: totals
   int3 tot = make_int3(0, 0, 0);
-  for (int i = i0 + threadIdx.x; i < i1; i += blockDim.x) tot = add3(tot, entry(i));
+  for (int i = i0 + threadIdx.x; i < i1; i += blockDim.x) tot = tot + entry(i);
   int3 all;
-  block_scan3(tot, sh3, &all);
+  block_inclusive_scan<int3, kAccWarps>(tot, sh3, &all);
   if (threadIdx.x == 0) *rec = all.z ? __ddiv_rn((double)all.x, npd) : 0.0;
   for (int r = threadIdx.x; r < R; r += blockDim.x) prec[r * rstride] = 0.0;  // thresholds past the last recall
   __syncthreads();
@@ -255,14 +221,14 @@ __global__ void __launch_bounds__(kAccTPB) coco_accumulate_kernel(
     const int i = i0 + c * kAccTPB + threadIdx.x;
     const int3 e = entry(i);
     int3 chunk;
-    const int3 incl = block_scan3(e, sh3, &chunk);
+    const int3 incl = block_inclusive_scan<int3, kAccWarps>(e, sh3, &chunk);
     // counts up to and including i over the whole segment
     const int tp = all.x - after.x - chunk.x + incl.x;
     const int fp = all.y - after.y - chunk.y + incl.y;
     const int kept_before = all.z - after.z - chunk.z + incl.z - e.z;
     const double tpd = (double)tp;
     const double pr = e.z ? __ddiv_rn(tpd, __dadd_rn(__dadd_rn((double)fp, tpd), DBL_EPSILON)) : -1.0;
-    const double suf = fmax(block_suffix_max(pr, shd), carry_max);
+    const double suf = fmax(block_suffix_max<kAccWarps>(pr, shd), carry_max);
     if (e.z) {
       const double rc = __ddiv_rn(tpd, npd);
       const int lo = kept_before == 0 ? 0 : upper_bound(s_thr, R, __ddiv_rn((double)(tp - e.x), npd));
@@ -273,16 +239,9 @@ __global__ void __launch_bounds__(kAccTPB) coco_accumulate_kernel(
     if (threadIdx.x == 0) shd[0] = suf;
     __syncthreads();
     carry_max = shd[0];
-    after = add3(after, chunk);
+    after = after + chunk;
     __syncthreads();
   }
-}
-
-bool monotone(const int* off, int n) {
-  if (off[0] != 0) return false;
-  for (int i = 0; i < n; ++i)
-    if (off[i + 1] < off[i]) return false;
-  return true;
 }
 
 }  // namespace
@@ -295,8 +254,8 @@ int sniper_coco_box_iou_batched(const double* dt_box, const double* gt_box, cons
   SN_CHECK(P >= 0, "coco_box_iou_batched: P (%d) must not be negative", P);
   if (P == 0) return 0;
   SN_CHECK(dt_off_host && gt_off_host && iou_off_host, "coco_box_iou_batched: the host offsets must not be null");
-  SN_CHECK(monotone(dt_off_host, P), "coco_box_iou_batched: dt_off must start at 0 and not decrease");
-  SN_CHECK(monotone(gt_off_host, P), "coco_box_iou_batched: gt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(dt_off_host, P), "coco_box_iou_batched: dt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(gt_off_host, P), "coco_box_iou_batched: gt_off must start at 0 and not decrease");
   SN_CHECK(iou_off_host[0] == 0, "coco_box_iou_batched: iou_off must start at 0");
   for (int p = 0; p < P; ++p) {
     const long n = (long)(dt_off_host[p + 1] - dt_off_host[p]) * (gt_off_host[p + 1] - gt_off_host[p]);
@@ -324,8 +283,8 @@ int sniper_coco_match(const double* dt_box, const double* dt_area, const long* d
   SN_CHECK(iou_thrs && area_rng, "coco_match: iou_thrs / area_rng (host) must not be null");
   if (P == 0) return 0;
   SN_CHECK(dt_off_host && gt_off_host, "coco_match: the host offsets must not be null");
-  SN_CHECK(monotone(dt_off_host, P), "coco_match: dt_off must start at 0 and not decrease");
-  SN_CHECK(monotone(gt_off_host, P), "coco_match: gt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(dt_off_host, P), "coco_match: dt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(gt_off_host, P), "coco_match: gt_off must start at 0 and not decrease");
   const long Dtot = dt_off_host[P], Gtot = gt_off_host[P];
   SN_CHECK(dt_off && gt_off && npig, "coco_match: dt_off / gt_off / npig must not be null");
   SN_CHECK(Dtot == 0 || (dt_box && dt_area && dt_id && dt_flags),
@@ -362,9 +321,9 @@ int sniper_coco_accumulate(const unsigned char* dt_flags, const int* dt_rank, co
     SN_CHECK(rec_thrs[i] <= rec_thrs[i + 1], "coco_accumulate: recThrs must be sorted (index %d)", i);
   if (K == 0) return 0;
   SN_CHECK(cat_pair_off_host && dt_off_host, "coco_accumulate: the host offsets must not be null");
-  SN_CHECK(monotone(cat_pair_off_host, K) && cat_pair_off_host[K] == P,
+  SN_CHECK(sn::offsets_ok(cat_pair_off_host, K) && cat_pair_off_host[K] == P,
            "coco_accumulate: cat_pair_off must start at 0, not decrease and end at P (%d)", P);
-  SN_CHECK(monotone(dt_off_host, P), "coco_accumulate: dt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(dt_off_host, P), "coco_accumulate: dt_off must start at 0 and not decrease");
   SN_CHECK(cat_pair_off && dt_off && (npig || P == 0), "coco_accumulate: cat_pair_off / dt_off / npig must not be null");
   SN_CHECK(dt_off_host[P] == 0 || (dt_flags && dt_rank && cat_order),
            "coco_accumulate: dt_flags / dt_rank / cat_order must not be null");

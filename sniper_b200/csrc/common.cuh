@@ -33,6 +33,15 @@ void set_error(const char* fmt, ...);
 
 static inline int div_up(long a, long b) { return (int)((a + b - 1) / b); }
 
+// a host offset array off[0 .. n] (int or long long) that starts at 0 and never decreases
+template <typename T>
+bool offsets_ok(const T* off, long n) {
+  if (off[0] != 0) return false;
+  for (long i = 0; i < n; ++i)
+    if (off[i + 1] < off[i]) return false;
+  return true;
+}
+
 constexpr int kNumSMs = 132;   // H100 SXM
 
 // Caller-owned device scratch, one buffer per (device, stream) registered with sniper_set_stream_workspace: launches on

@@ -17,6 +17,7 @@
 // one grid-wide barrier, and writes at offsets given by the exclusive scan of the counts, so the buffer holds the
 // rows in (chip, roi, class) order whatever the block schedule.
 #include "common.cuh"
+#include "np_pairwise.cuh"
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -31,10 +32,6 @@ constexpr int kChipCols = 12;   // image, chip id, chip x1 y1 x2 y2, image width
 
 // key = image:19 | class:10 | scale:4 | chip:14 | roi:16 (63 bits: sorts the same signed or unsigned)
 constexpr int kRoiBits = 16, kChipBits = 14, kScaleBits = 4, kClassBits = 10;
-
-// np.minimum / np.maximum: a NaN operand is returned
-__device__ __forceinline__ double np_min(double a, double b) { return (a != a) ? a : ((b != b) ? b : (a < b ? a : b)); }
-__device__ __forceinline__ double np_max(double a, double b) { return (a != a) ? a : ((b != b) ? b : (a > b ? a : b)); }
 
 struct Args {
   const float* rois;

@@ -21,6 +21,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "block_reduce.cuh"
 #include "common.cuh"
 
 namespace {
@@ -60,16 +61,6 @@ __device__ void unite(int* lab, int a, int b) {
       done = true;
     }
   } while (!done);
-}
-
-__device__ int block_sum(int v, int* s_red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(~0u, v, o);
-  __syncthreads();                               // s_red of an earlier call has been read
-  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  int t = 0;
-  for (int w = 0; w < kWarps; ++w) t += s_red[w];
-  return t;
 }
 
 struct Scratch {
@@ -119,7 +110,7 @@ __device__ int label_pass(const Scratch& s, int* s_red) {
       ++cnt;
     }
   }
-  return block_sum(cnt, s_red);
+  return block_sum<int, kWarps>(cnt, s_red);
 }
 
 struct Rect {

@@ -16,6 +16,7 @@
 // positions [0, live) at the end are the reference's returned array.  Arithmetic follows the Cythonized reference
 // (float IoU with the `+ 1` sums evaluated in double and narrowed once, Gaussian weight = exp evaluated in double);
 // this file is compiled with -fmad=false.
+#include "block_reduce.cuh"
 #include "common.cuh"
 #include <limits.h>
 #include <math.h>
@@ -50,19 +51,14 @@ __global__ void __launch_bounds__(kNmsTPB) soft_nms_batched_kernel(float* __rest
       const float s = work[5 * q + 4];
       if (s > best) { best = s; bq = q; }          // strict >: the lowest position wins a tie within a thread
     }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, off);
-      const int oq = __shfl_xor_sync(0xffffffffu, bq, off);
-      if (ob > best || (ob == best && oq < bq)) { best = ob; bq = oq; }
-    }
+    warp_argmax(best, bq);
     if (lane == 0) { s_val[warp] = best; s_pos[warp] = bq; }
     __syncthreads();
     if (tid == 0) {
       float b = s_val[0];
       int k = s_pos[0];
       for (int w = 1; w < kNmsWarps; ++w)
-        if (s_val[w] > b || (s_val[w] == b && s_pos[w] < k)) { b = s_val[w]; k = s_pos[w]; }
+        if (argmax_beats(s_val[w], s_pos[w], b, k)) { b = s_val[w]; k = s_pos[w]; }
       s_stop = k == INT_MAX;                       // only scores the contract rules out (NaN, <= -1) remain
       if (!s_stop) {
 #pragma unroll

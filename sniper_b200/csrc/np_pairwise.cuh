@@ -1,9 +1,14 @@
 // numpy's pairwise summation of a contiguous float64 array (np.sum / np.mean's reduction), restated for one device
-// thread.  Shared by the evaluations whose results are graded byte-equal with numpy: include it only in translation
-// units built with -fmad=false.
+// thread, and np.maximum / np.minimum of two doubles.  Shared by the evaluations whose results are graded byte-equal
+// with numpy: include it only in translation units built with -fmad=false.
 #pragma once
 
 namespace {
+
+// np.maximum / np.minimum: a NaN operand is the result (a when both are); otherwise the larger / smaller, and b when
+// they compare equal (np.maximum(-0.0, 0.0) is 0.0).  A NaN b fails the compare and is returned.
+__device__ __forceinline__ double np_max(double a, double b) { return (a != a || a > b) ? a : b; }
+__device__ __forceinline__ double np_min(double a, double b) { return (a != a || a < b) ? a : b; }
 
 constexpr int kPwBlock = 128;  // numpy's PW_BLOCKSIZE
 constexpr int kPwDepth = 48;

@@ -15,6 +15,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "block_reduce.cuh"
 #include "common.cuh"
 #include "np_pairwise.cuh"
 
@@ -27,6 +28,7 @@ constexpr int kMaxCols = 1024;                  // GTs of one (image, range) pai
 constexpr long kSmemCap = 110 * 1024;           // dynamic shared memory of a matching block: two blocks per SM
 constexpr int kColBytes = 6 * 8 + 2 * 4;        // box[4], area, best value; best row, used
 constexpr int kAccTPB = 256;
+constexpr int kAccWarps = kAccTPB / 32;
 constexpr int kAccChunk = 2048;                 // gt_overlaps values a counting block stages in shared memory
 
 // matching status per pair: the reference's assert (a best overlap < 0 or NaN) and the ZeroDivisionError of
@@ -48,18 +50,6 @@ __device__ __forceinline__ double widen(T v) { return (double)v; }
 // cython's min / max of two C doubles: the second argument when it compares strictly less / greater
 __device__ __forceinline__ double cy_min(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double cy_max(double a, double b) { return b > a ? b : a; }
-
-// (value, row) order of the reference's argmax: the larger value, the lower index on ties; NaN never enters (it is an
-// error before any round)
-__device__ __forceinline__ bool better(double v, int r, double bv, int br) { return v > bv || (v == bv && r < br); }
-
-__device__ __forceinline__ void warp_best(double* v, int* r) {
-  for (int o = 16; o > 0; o >>= 1) {
-    const double ov = __shfl_xor_sync(~0u, *v, o);
-    const int orow = __shfl_xor_sync(~0u, *r, o);
-    if (better(ov, orow, *v, *r)) { *v = ov; *r = orow; }
-  }
-}
 
 struct MatchParams {
   int num_images, pair_begin;
@@ -163,7 +153,7 @@ __global__ void __launch_bounds__(kMatchTPB, 2) recall_match_kernel(
       nan_seen |= isnan(v);
       if (v > bv || br == INT_MAX) { bv = v; br = row; }
     }
-    warp_best(&bv, &br);
+    warp_argmax(bv, br);
     if (lane == 0) { cbest[j] = bv; crow[j] = br; }
   }
   if (__syncthreads_or(nan_seen)) {
@@ -177,8 +167,8 @@ __global__ void __launch_bounds__(kMatchTPB, 2) recall_match_kernel(
       double bv = -INFINITY;
       int bj = INT_MAX;
       for (int j = lane; j < m; j += 32)
-        if (!cused[j] && better(cbest[j], j, bv, bj)) { bv = cbest[j]; bj = j; }
-      warp_best(&bv, &bj);
+        if (!cused[j] && argmax_beats(cbest[j], j, bv, bj)) { bv = cbest[j]; bj = j; }
+      warp_argmax(bv, bj);
       if (lane == 0) {
         // assert (gt_ovr >= 0)
         if (!(bv >= 0.0)) {
@@ -204,9 +194,9 @@ __global__ void __launch_bounds__(kMatchTPB, 2) recall_match_kernel(
       int br = INT_MAX;
       for (int row = lane; row < n; row += 32) {
         const double v = mat[(long)j * n + row];
-        if (v > bv || (v == bv && row < br)) { bv = v; br = row; }
+        if (argmax_beats(v, row, bv, br)) { bv = v; br = row; }
       }
-      warp_best(&bv, &br);
+      warp_argmax(bv, br);
       if (lane == 0) { cbest[j] = bv; crow[j] = br; }
     }
     __syncthreads();
@@ -220,17 +210,6 @@ struct AccParams {
   long long num_props;
   int T, prop_dtype, count_blocks, num_images;
 };
-
-__device__ __forceinline__ unsigned long long block_sum(unsigned long long v, unsigned long long* sh) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(~0u, v, o);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  unsigned long long s = 0;
-  for (int w = 0; w < kAccTPB / 32; ++w) s += sh[w];
-  return s;
-}
 
 // area_ranges[1:] of the reference as bounds in the box dtype: >= lo and < hi
 __device__ int hist_bin_u16(const uint16_t* b) {
@@ -269,7 +248,7 @@ __global__ void __launch_bounds__(kAccTPB) recall_accumulate_kernel(
     const AccParams prm, unsigned long long* __restrict__ counts, unsigned int* __restrict__ done,
     double* __restrict__ recalls, double* __restrict__ ar, double* __restrict__ hist) {
   __shared__ double sv[kAccChunk];
-  __shared__ unsigned long long sh[kAccTPB / 32];
+  __shared__ unsigned long long sh[kAccWarps];
   __shared__ bool s_last;
   const int T = prm.T;
   if ((int)blockIdx.x < prm.count_blocks) {
@@ -293,7 +272,7 @@ __global__ void __launch_bounds__(kAccTPB) recall_accumulate_kernel(
       const double th = thr[t];
       unsigned long long c = 0;
       for (int k = threadIdx.x; k < len; k += kAccTPB) c += sv[k] >= th;
-      c = block_sum(c, sh);
+      c = block_sum<unsigned long long, kAccWarps>(c, sh);
       if (threadIdx.x == 0 && c) atomicAdd(&counts[(long)r * T + t], c);
     }
   } else {
@@ -308,7 +287,7 @@ __global__ void __launch_bounds__(kAccTPB) recall_accumulate_kernel(
       for (int j = 0; j < 6; ++j) c[j] += k == j;
     }
     for (int j = 0; j < 6; ++j) {
-      const unsigned long long s = block_sum(c[j], sh);
+      const unsigned long long s = block_sum<unsigned long long, kAccWarps>(c[j], sh);
       if (threadIdx.x == 0 && s) atomicAdd(&counts[(long)kRanges * T + j], s);
     }
   }
@@ -335,13 +314,6 @@ __global__ void __launch_bounds__(kAccTPB) recall_accumulate_kernel(
   }
 }
 
-bool monotone(const int* off, int n) {
-  if (off[0] != 0) return false;
-  for (int i = 0; i < n; ++i)
-    if (off[i + 1] < off[i]) return false;
-  return true;
-}
-
 // per pair: n, m; -1 with the message set when the inputs are refused
 int pair_sizes(const int* prop_off_host, const int* gt_off_host, const unsigned char* gt_range_host, int num_images,
                int* pair_n, int* pair_m) {
@@ -363,8 +335,8 @@ int check_csr(const int* prop_off_host, const int* gt_off_host, const unsigned c
   SN_CHECK(num_images >= 0, "proposal_recall: num_images (%d) must not be negative", num_images);
   SN_CHECK((long)num_images * kRanges < INT_MAX, "proposal_recall: num_images (%d) is too large", num_images);
   SN_CHECK(prop_off_host && gt_off_host, "proposal_recall: the host offsets must not be null");
-  SN_CHECK(monotone(prop_off_host, num_images), "proposal_recall: prop_off must start at 0 and not decrease");
-  SN_CHECK(monotone(gt_off_host, num_images), "proposal_recall: gt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(prop_off_host, num_images), "proposal_recall: prop_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(gt_off_host, num_images), "proposal_recall: gt_off must start at 0 and not decrease");
   SN_CHECK(gt_off_host[num_images] == 0 || gt_range_host, "proposal_recall: gt_range (host) must not be null");
   for (int g = 0; g < gt_off_host[num_images]; ++g)
     SN_CHECK(gt_range_host[g] < (1u << kRanges), "proposal_recall: gt_range[%d] (%d) has bits above the %d ranges", g,
@@ -473,10 +445,9 @@ int sniper_proposal_recall_accumulate(const double* gt_overlaps, const long long
            "not be negative", num_props, num_images);
   SN_CHECK(range_off_host && num_pos_host, "proposal_recall_accumulate: range_off / num_pos (host) must not be null");
   SN_CHECK(range_off_host[0] == 0, "proposal_recall_accumulate: range_off must start at 0");
-  for (int r = 0; r < kRanges; ++r) {
-    SN_CHECK(range_off_host[r + 1] >= range_off_host[r], "proposal_recall_accumulate: range_off must not decrease");
+  SN_CHECK(sn::offsets_ok(range_off_host, kRanges), "proposal_recall_accumulate: range_off must not decrease");
+  for (int r = 0; r < kRanges; ++r)
     SN_CHECK(num_pos_host[r] >= 0, "proposal_recall_accumulate: num_pos[%d] must not be negative", r);
-  }
   SN_CHECK(counts && done && ar && hist, "proposal_recall_accumulate: counts / done / ar / hist must not be null");
   SN_CHECK(T == 0 || (thresholds && recalls), "proposal_recall_accumulate: thresholds / recalls must not be null");
   SN_CHECK(range_off_host[kRanges] == 0 || gt_overlaps, "proposal_recall_accumulate: gt_overlaps must not be null");

@@ -17,6 +17,7 @@
 // captured graph can be replayed).  Two runs give byte-identical accumulators.  The L1 sums are read from the loss
 // buffer the smooth-L1 loss kernels filled with float atomics and inherit their last-bit run-to-run variation.
 // This file is compiled with -fmad=false.
+#include "block_reduce.cuh"
 #include "common.cuh"
 #include <math.h>
 
@@ -24,7 +25,8 @@ namespace {
 
 constexpr int kTmTPB = 256;
 constexpr int kTmWarps = kTmTPB / 32;
-constexpr int kTmMaxBlocks = 8 * sn::kNumSMs;   // a full wave at 256 threads: the anchor loop is latency-bound
+constexpr int kTmBlocksPerSM = 8;              // the launch bound keeps the registers low enough for 8 to fit
+constexpr int kTmMaxBlocks = kTmBlocksPerSM * sn::kNumSMs;   // one full wave: the anchor loop is latency-bound
 constexpr int kSlots = 8;
 
 struct Partial {
@@ -76,21 +78,7 @@ __device__ __forceinline__ void two_way(const float* __restrict__ prob, int ld, 
   }
 }
 
-template <typename T>
-__device__ __forceinline__ T block_sum(T v, T* sh) {
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  T s = 0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < kTmWarps; ++w) s += sh[w];
-  return s;   // meaningful in thread 0 only
-}
-
-__global__ void __launch_bounds__(kTmTPB) train_metric_kernel(Args a) {
+__global__ void __launch_bounds__(kTmTPB, kTmBlocksPerSM) train_metric_kernel(Args a) {
   __shared__ double shd[kTmWarps];
   __shared__ long long shl[kTmWarps];
   __shared__ bool last;
@@ -111,12 +99,7 @@ __global__ void __launch_bounds__(kTmTPB) train_metric_kernel(Args a) {
       const float v = row[k];
       if (v > m) m = v, mi = k;              // strictly greater: the lane keeps its first maximum
     }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      const float om = __shfl_xor_sync(0xffffffffu, m, off);
-      const int oi = __shfl_xor_sync(0xffffffffu, mi, off);
-      if (om > m || (om == m && oi < mi)) m = om, mi = oi;
-    }
+    warp_argmax(m, mi);
     if (lane == 0) {
       hits[1] += (mi == l);
       loss[1] += log_term(row[l]);
@@ -124,8 +107,8 @@ __global__ void __launch_bounds__(kTmTPB) train_metric_kernel(Args a) {
   }
   Partial* mine = &a.ws->part[blockIdx.x];
   for (int j = 0; j < 3; ++j) {
-    const long long h = block_sum(hits[j], shl);
-    const double s = block_sum(loss[j], shd);
+    const long long h = block_sum<long long, kTmWarps>(hits[j], shl);
+    const double s = block_sum<double, kTmWarps>(loss[j], shd);
     if (threadIdx.x == 0) mine->hits[j] = h, mine->loss[j] = s;
   }
   __threadfence();

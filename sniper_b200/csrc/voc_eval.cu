@@ -14,6 +14,7 @@
 #include <limits.h>
 #include <math.h>
 
+#include "block_reduce.cuh"
 #include "common.cuh"
 #include "np_pairwise.cuh"
 
@@ -24,10 +25,6 @@ constexpr int kMax07 = 32;     // recall thresholds of the 11-point metric
 constexpr int kMatchTPB = 128;
 constexpr int kAccTPB = 256;
 constexpr int kAccWarps = kAccTPB / 32;
-
-// np.maximum / np.minimum: a NaN operand is the result
-__device__ __forceinline__ double np_max(double a, double b) { return (isnan(a) || a >= b) ? a : b; }
-__device__ __forceinline__ double np_min(double a, double b) { return (isnan(a) || a <= b) ? a : b; }
 
 struct MatchParams {
   double thr[kMaxT];
@@ -98,41 +95,6 @@ struct AccParams {
   long N;
 };
 
-__device__ __forceinline__ int2 add2(int2 a, int2 b) { return make_int2(a.x + b.x, a.y + b.y); }
-
-// inclusive block scan of (a, b) counts; *total gets the block's sum
-__device__ int2 block_scan2(int2 v, int2* sh, int2* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const int2 n = make_int2(__shfl_up_sync(~0u, v.x, o), __shfl_up_sync(~0u, v.y, o));
-    if (lane >= o) v = add2(v, n);
-  }
-  if (lane == 31) sh[warp] = v;
-  __syncthreads();
-  int2 before = make_int2(0, 0), all = make_int2(0, 0);
-  for (int w = 0; w < kAccWarps; ++w) {
-    if (w < warp) before = add2(before, sh[w]);
-    all = add2(all, sh[w]);
-  }
-  __syncthreads();
-  *total = all;
-  return add2(v, before);
-}
-
-// inclusive suffix max over the block (threads at and after this one); the values are never NaN
-__device__ double block_suffix_max(double v, double* sh) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 1; o < 32; o <<= 1) {
-    const double n = __shfl_down_sync(~0u, v, o);
-    if (lane + o < 32) v = fmax(v, n);
-  }
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  for (int w = warp + 1; w < kAccWarps; ++w) v = fmax(v, sh[w]);
-  __syncthreads();
-  return v;
-}
-
 // pascal_voc_eval.py:173-179 and voc_ap (:39-70) for one (class, threshold) per block.
 // Pass 1 (forward): the integer scans of tp / fp, rec = tp / float(npos), prec = tp / max(tp + fp, eps), the 11-point
 // maxima, and the count of positions where mrec = [0, rec, 1] changes.  Pass 2 (area metric, chunks from the end):
@@ -144,6 +106,7 @@ __global__ void __launch_bounds__(kAccTPB) voc_accumulate_kernel(const unsigned 
                                                                  double* __restrict__ rec, double* __restrict__ prec,
                                                                  double* __restrict__ ap, double* __restrict__ terms) {
   __shared__ int2 sh2[kAccWarps];
+  __shared__ int sh1[kAccWarps];
   __shared__ double shd[kAccWarps];
   __shared__ double s07[kAccWarps][kMax07];
   __shared__ int s_changed;
@@ -165,8 +128,8 @@ __global__ void __launch_bounds__(kAccTPB) voc_accumulate_kernel(const unsigned 
     const int i = ch * kAccTPB + threadIdx.x;
     const unsigned char f = i < n ? fl[i] : 0;
     int2 chunk;
-    const int2 incl = add2(block_scan2(make_int2(f == 1, f == 2), sh2, &chunk), before);
-    before = add2(before, chunk);
+    const int2 incl = block_inclusive_scan<int2, kAccWarps>(make_int2(f == 1, f == 2), sh2, &chunk) + before;
+    before = before + chunk;
     if (i < n) {
       const double tpd = (double)incl.x, fpd = (double)incl.y;
       const double r = __ddiv_rn(tpd, npd);
@@ -222,27 +185,20 @@ __global__ void __launch_bounds__(kAccTPB) voc_accumulate_kernel(const unsigned 
       r_prev = i == 0 ? 0.0 : rc[i - 1];
       ci = r != r_prev;
     }
-    const double mp = fmax(block_suffix_max(pr, shd), carry);
+    const double mp = fmax(block_suffix_max<kAccWarps>(pr, shd), carry);
     // changed positions at and after i within the chunk: an inclusive scan from the end
-    int2 tot;
-    const int2 incl = block_scan2(make_int2(ci, 0), sh2, &tot);
-    const int at_or_after = tot.x - incl.x + ci;
+    int tot;
+    const int incl = block_inclusive_scan<int, kAccWarps>(ci, sh1, &tot);
+    const int at_or_after = tot - incl + ci;
     if (ci) tm[s_changed - after - at_or_after] = __dmul_rn(__dsub_rn(r, r_prev), mp);
     if (threadIdx.x == 0) shd[0] = mp;
     __syncthreads();
     carry = shd[0];
-    after += tot.x;
+    after += tot;
     __syncthreads();
   }
   __syncthreads();
   if (threadIdx.x == 0) ap[(long)t * prm.C + c] = np_sum(tm, m);
-}
-
-bool monotone(const int* off, int n) {
-  if (off[0] != 0) return false;
-  for (int i = 0; i < n; ++i)
-    if (off[i + 1] < off[i]) return false;
-  return true;
 }
 
 }  // namespace
@@ -258,8 +214,8 @@ int sniper_voc_match(const double* det_box, const int* pair_det_off, const int* 
   SN_CHECK(thresholds, "voc_match: thresholds (host) must not be null");
   if (P == 0) return 0;
   SN_CHECK(pair_det_off_host && gt_off_host, "voc_match: the host offsets must not be null");
-  SN_CHECK(monotone(pair_det_off_host, P), "voc_match: pair_det_off must start at 0 and not decrease");
-  SN_CHECK(monotone(gt_off_host, P), "voc_match: gt_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(pair_det_off_host, P), "voc_match: pair_det_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(gt_off_host, P), "voc_match: gt_off must start at 0 and not decrease");
   const long N = pair_det_off_host[P], G = gt_off_host[P];
   SN_CHECK(pair_det_off && gt_off, "voc_match: pair_det_off / gt_off must not be null");
   SN_CHECK(N == 0 || (det_box && pair_det_pos && flags), "voc_match: det_box / pair_det_pos / flags must not be null");
@@ -289,7 +245,7 @@ int sniper_voc_accumulate(const unsigned char* flags, const int* det_off, const 
   }
   if (C == 0) return 0;
   SN_CHECK(det_off_host, "voc_accumulate: the host offsets must not be null");
-  SN_CHECK(monotone(det_off_host, C), "voc_accumulate: det_off must start at 0 and not decrease");
+  SN_CHECK(sn::offsets_ok(det_off_host, C), "voc_accumulate: det_off must start at 0 and not decrease");
   const long N = det_off_host[C];
   SN_CHECK(det_off && npos && ap, "voc_accumulate: det_off / npos / ap must not be null");
   SN_CHECK(N == 0 || (flags && rec && prec), "voc_accumulate: flags / rec / prec must not be null");
