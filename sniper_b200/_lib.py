@@ -75,6 +75,7 @@ SIGNATURES = {
     "sniper_chip_input": ("i", "ppppiip"),
     "sniper_chip_input_hw": ("i", "ppppiiip"),
     "sniper_anchor_subsample": ("i", "pppiiiiiiup"),
+    "sniper_anchor_subsample_at": ("i", "pppiiiiiiuip"),
     "sniper_chips_generate": ("i", "piiiiipi"),
     "sniper_cpu_nms": ("i", "ppidp"),
     "sniper_cpu_soft_nms": ("i", "pifffu"),

@@ -53,10 +53,11 @@ class Speedometer(object):
 def module_checkpoint(trainer, prefix, period=1, save_optimizer_states=True):
     """Epoch-end callback: every `period` epochs, `<prefix>-%04d.params` for epoch + 1 (with the `*_test` tensors of
     checkpoint_callback), `<prefix>-symbol.json` when the net was bound from a Symbol, and with save_optimizer_states
-    `<prefix>-%04d.states` (Trainer.save_checkpoint)."""
+    `<prefix>-%04d.states` (Trainer.save_checkpoint), from the arg / aux params fit passes."""
     period = int(max(1, period))
 
     def _callback(iter_no, sym=None, arg=None, aux=None):
         if (iter_no + 1) % period == 0 and _rank0():
-            trainer.save_checkpoint(prefix, iter_no + 1, save_optimizer_states)
+            # arg / aux: what fit exported on every rank (moving statistics averaged over the ranks)
+            trainer.save_checkpoint(prefix, iter_no + 1, save_optimizer_states, arg_params=arg, aux_params=aux)
     return _callback

@@ -56,17 +56,20 @@ class chip_generator(object):
 
 
 class chip_worker(object):
-    def __init__(self, cfg, chip_size):
+    def __init__(self, cfg, chip_size, rng=None):
+        """rng: a np.random.RandomState the chip stride is drawn from (default: the global np.random, as the
+        reference)."""
         self.valid_ranges = cfg.TRAIN.VALID_RANGES
         self.scales = cfg.TRAIN.SCALES
         self.chip_size = chip_size
         self.use_cpp = cfg.TRAIN.CPP_CHIPS
         self.use_neg_chips = cfg.TRAIN.USE_NEG_CHIPS
+        self.rng = rng
         self.reset()
 
     def reset(self):
         """A new chip stride per epoch (data_workers.py:380, 390-392)."""
-        self.chip_stride = np.random.randint(56, 60)
+        self.chip_stride = (np.random if self.rng is None else self.rng).randint(56, 60)
         self.chip_generator = chip_generator(chip_stride=self.chip_stride, use_cpp=self.use_cpp)
 
     # ---- helpers

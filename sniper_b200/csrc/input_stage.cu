@@ -127,12 +127,14 @@ __device__ void radix_select(const float* lab, int n, float cls, uint32_t seed, 
 
 __global__ void __launch_bounds__(kSubTPB) anchor_subsample_kernel(float* __restrict__ label, float* __restrict__ bbox_target,
                                                                     float* __restrict__ bbox_weight, int n, int A,
-                                                                    int HW, int num_fg, int batch_size, uint32_t seed) {
+                                                                    int HW, int num_fg, int batch_size, uint32_t seed,
+                                                                    int chip_base) {
   __shared__ int hist[256];
   __shared__ int sh[2];
   __shared__ int cnt[2];
   __shared__ int eq_taken;
   const int b = blockIdx.x;
+  const uint32_t chip = (uint32_t)(chip_base + b);      // the hash key: the chip's position in the global batch
   float* lab = label + (long)b * n;
   for (int cls = 1; cls >= 0; --cls) {
     if (threadIdx.x < 2) cnt[threadIdx.x] = 0;
@@ -154,14 +156,14 @@ __global__ void __launch_bounds__(kSubTPB) anchor_subsample_kernel(float* __rest
     const int drop = have - keep;
     uint32_t thr;
     int take_eq;
-    radix_select(lab, n, (float)cls, seed + (uint32_t)cls * 0x51ED27u, (uint32_t)b, drop, thr, take_eq, hist, sh);
+    radix_select(lab, n, (float)cls, seed + (uint32_t)cls * 0x51ED27u, chip, drop, thr, take_eq, hist, sh);
     // keys below the threshold go; of the keys EQUAL to it (a 32-bit collision exactly at the threshold: probability
     // ~n / 2^32) the first take_eq to arrive go
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const float l = lab[i];
       bool kill = false;
       if (l == (float)cls) {
-        const uint32_t key = mix32(seed + (uint32_t)cls * 0x51ED27u, (uint32_t)b, (uint32_t)i);
+        const uint32_t key = mix32(seed + (uint32_t)cls * 0x51ED27u, chip, (uint32_t)i);
         if (key < thr) kill = true;
         else if (key == thr) kill = atomicAdd(&eq_taken, 1) < take_eq;
       }
@@ -213,11 +215,22 @@ int sniper_chip_input_hw(const void* src, const void* table, const float* means_
 
 // label [B, A*H*W] in (a,h,w) order, bbox_target / bbox_weight [B,4A,H,W] (as sniper_anchor_target writes them), in
 // place.  Keeps <= num_fg positives and <= batch_size - #positives negatives per chip, chosen by hash(seed, chip, anchor).
+int sniper_anchor_subsample_at(float* label, float* bbox_target, float* bbox_weight, int B, int A, int H, int W,
+                               int num_fg, int batch_size, unsigned seed, int chip_base, void* stream);
+
 int sniper_anchor_subsample(float* label, float* bbox_target, float* bbox_weight, int B, int A, int H, int W, int num_fg,
                             int batch_size, unsigned seed, void* stream) {
+  return sniper_anchor_subsample_at(label, bbox_target, bbox_weight, B, A, H, W, num_fg, batch_size, seed, 0, stream);
+}
+
+// The same for chips [chip_base, chip_base + B) of a larger batch: chip b draws with the key of chip chip_base + b, so a
+// data-parallel rank that holds a slice of the global batch subsamples exactly what the whole batch in one launch would.
+int sniper_anchor_subsample_at(float* label, float* bbox_target, float* bbox_weight, int B, int A, int H, int W,
+                               int num_fg, int batch_size, unsigned seed, int chip_base, void* stream) {
   SN_CHECK(B > 0 && num_fg >= 0 && batch_size >= num_fg, "anchor_subsample: bad sizes");
+  SN_CHECK(chip_base >= 0, "anchor_subsample: chip_base must not be negative");
   anchor_subsample_kernel<<<B, kSubTPB, 0, (cudaStream_t)stream>>>(label, bbox_target, bbox_weight, A * H * W, A, H * W,
-                                                                  num_fg, batch_size, seed);
+                                                                  num_fg, batch_size, seed, chip_base);
   SN_LAUNCH_CHECK();
   return 0;
 }

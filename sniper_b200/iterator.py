@@ -14,7 +14,14 @@ Device side (`InputStage`): one H2D copy of that raw batch, then `sniper_chip_in
 provide_label` name: data, valid_ranges, im_info, label, bbox_target, bbox_weight, gt_boxes (SURVEY appendix B.5).
 
 What stays on the host is what north_star keeps there: lib/chips sampling and the iterator's index logic.
+
+Data parallel (`rank=`): the reference builds ONE iterator over the global batch of nGPUs * BATCH_IMAGES chips and MXNet
+hands GPU g the slice [g*B, (g+1)*B) of every batch (executor_manager._split_input_slice).  Here every rank runs its
+own iterator over the same roidb with the same `seed`: each computes the whole epoch plan, identically, and builds only
+its own slice.  `RawBatch.chip_base` carries the slice's position, so the device subsampling draws what the global
+batch would (`sniper_anchor_subsample_at`), and `RawBatch.plan_digest` lets Trainer.fit check that the ranks agree.
 """
+import hashlib
 import math
 
 import numpy as np
@@ -118,6 +125,8 @@ class RawBatch(object):
         self.anchor_im_info = pin(B, 3, dtype=torch.float32)
         self.used_pixels = 0
         self.seed = 0
+        self.chip_base = 0           # position of chip 0 of this batch in the global batch (data parallel: rank * B)
+        self.plan_digest = None      # 64-bit digest of the epoch plan the batch comes from (MNIteratorE2E.plan_digest)
 
     def nbytes(self):
         small = (self.table, self.valid_ranges, self.im_info, self.gt_valid, self.ngt, self.gt_invalid, self.ninv,
@@ -127,20 +136,52 @@ class RawBatch(object):
         return int(self.used_pixels + sum(t.numel() * t.element_size() for t in small))
 
 
+def roidb_digest(roidb):
+    """64-bit digest of a training roidb: its size and, per entry, the image path, size, flip and boxes."""
+    h = hashlib.blake2b(digest_size=8)
+    h.update(np.int64(len(roidb)).tobytes())
+    for r in roidb:
+        h.update(str(r.get('image', '')).encode())
+        h.update(np.array([r['width'], r['height'], bool(r.get('flipped', False))], np.int64).tobytes())
+        h.update(np.ascontiguousarray(r['boxes'], np.float64).tobytes())
+    return int.from_bytes(h.digest(), 'little')
+
+
 class MNIteratorE2E(object):
     def __init__(self, roidb, config, batch_size=4, threads=8, nGPUs=1, pad_rois_to=400, crop_size=(512, 512),
-                 image_loader=None, n_buffers=3):
+                 image_loader=None, n_buffers=3, rank=None, seed=None):
         """roidb entries: 'image' (path) or 'image_data' (decoded uint8 HxWx3 BGR), 'width', 'height', 'boxes' [n,4],
         'max_overlaps' (== 1 for GT rows), 'max_classes', 'flipped'.  image_loader(path) -> uint8 BGR array replaces
-        cv2.imread (this image has no OpenCV)."""
+        cv2.imread (this image has no OpenCV).
+
+        batch_size is the GLOBAL batch (nGPUs * TRAIN.BATCH_IMAGES, main_train.py:44-45).  rank=None yields whole
+        batches; rank=r (data parallel, one iterator per rank) yields batches of B = batch_size // nGPUs chips, chips
+        [r*B, (r+1)*B) of the global batch the rank=None iterator with the same seed yields.  Every rank computes the
+        whole epoch plan (chips, padding, permutation, chip order), so len() and the epoch length are the global ones.
+        seed=int: every draw of an epoch comes from a private np.random.RandomState(seed) -- the chip stride, the
+        negative-chip pick, the chip permutation, each image's chip_order -- and each epoch seeds the C rand() stream
+        of the chip generator from it; seed=None draws from the global np.random (the reference's behaviour).  rank
+        needs a seed: the plan is computed on the prefetch thread, where the global state cannot be shared."""
         assert batch_size % nGPUs == 0, 'batch_size should be divisible by number of GPUs'
+        if rank is not None:
+            if seed is None:
+                raise ValueError("MNIteratorE2E: rank=%r needs a seed (every rank must draw the same epoch plan)" % rank)
+            if not 0 <= rank < nGPUs:
+                raise ValueError("MNIteratorE2E: rank %r is not in [0, nGPUs = %d)" % (rank, nGPUs))
         self.roidb = roidb
         self.cfg = config
         self.batch_size = batch_size
+        self.nGPUs = nGPUs
+        self.rank = rank
+        self.slice_size = batch_size if rank is None else batch_size // nGPUs
+        self.chip_base = 0 if rank is None else rank * self.slice_size
+        self.rng = None if seed is None else np.random.RandomState(seed)
+        self._roidb_digest = roidb_digest(roidb)
+        self.plan_digest = None
         self.crop_size = crop_size
         self.image_loader = image_loader
         self.pixel_mean = config.network.PIXEL_MEANS
-        self.chip_worker = chip_worker(chip_size=self.crop_size[0], cfg=config)
+        self.chip_worker = chip_worker(chip_size=self.crop_size[0], cfg=config, rng=self.rng)
         self.max_gt = 100
         self.data_name = ['data', 'valid_ranges', 'im_info']
         self.label_name = ['label', 'bbox_target', 'bbox_weight', 'gt_boxes']
@@ -160,10 +201,13 @@ class MNIteratorE2E(object):
 
     # ---------------------------------------------------------------- epoch (MNIteratorE2E.py:41-105)
     def reset(self):
+        npr = np.random if self.rng is None else self.rng
         self.cur_i = 0
         self.n_neg_per_im = 2
         self.crop_idx = [0] * len(self.roidb)
         self.chip_worker.reset()
+        if self.rng is not None:
+            host.srand(int(self.rng.randint(0, 2 ** 31)))
         chip_count = 0
         for r in self.roidb:
             r['crops'] = self.chip_worker.chip_extractor(r)
@@ -181,7 +225,7 @@ class MNIteratorE2E(object):
                 if len(cs) > 0:
                     sel_inds = np.arange(len(cs))
                     if len(cs) > self.n_neg_per_im:
-                        sel_inds = np.random.permutation(sel_inds)[0:self.n_neg_per_im]
+                        sel_inds = npr.permutation(sel_inds)[0:self.n_neg_per_im]
                     for ind in sel_inds:
                         chip_count += 1
                         r['crops'].append(r['neg_crops'][ind])
@@ -192,11 +236,24 @@ class MNIteratorE2E(object):
         if chipindex.shape[0] % self.batch_size > 0:
             extra = self.batch_size - (chipindex.shape[0] % self.batch_size)
             chipindex = np.hstack((chipindex, chipindex[0:extra]))
-        self.inds = np.array(np.random.permutation(chipindex), dtype=int)
+        self.inds = np.array(npr.permutation(chipindex), dtype=int)
         for r in self.roidb:
-            r['chip_order'] = np.random.permutation(np.arange(len(r['crops'])))
+            r['chip_order'] = npr.permutation(np.arange(len(r['crops'])))
         self.epiter += 1
         self.size = len(self.inds)
+        self.plan_digest = self._digest()
+
+    def _digest(self):
+        """64-bit digest of this epoch's plan: the roidb (roidb_digest), the chip stride, the chip count, the padded
+        chip permutation `inds`, and every image's chips and chip order."""
+        h = hashlib.blake2b(digest_size=8)
+        h.update(np.array([self._roidb_digest, self.chip_worker.chip_stride, self.chip_count, len(self.inds)],
+                          np.uint64).tobytes())
+        h.update(np.ascontiguousarray(self.inds, np.int64).tobytes())
+        for r in self.roidb:
+            h.update(np.array([c[0] for c in r['crops']], np.float64).tobytes())
+            h.update(np.ascontiguousarray(r['chip_order'], np.int64).tobytes())
+        return int.from_bytes(h.digest(), 'little')
 
     def __len__(self):
         return len(self.inds)
@@ -231,7 +288,7 @@ class MNIteratorE2E(object):
         self._next_buffer = (i + 1) % len(self._buffers)
         buf = self._buffers[i]
         if buf is None or buf.pixels.numel() < need_pixels:
-            buf = self._buffers[i] = RawBatch(self.batch_size, self.max_gt, int(need_pixels * 1.25) + 4096,
+            buf = self._buffers[i] = RawBatch(self.slice_size, self.max_gt, int(need_pixels * 1.25) + 4096,
                                               self.focus_cap)
         return buf
 
@@ -242,6 +299,9 @@ class MNIteratorE2E(object):
                    for r, i in zip(entries, range(cur_from, cur_to))]
         for i in range(cur_from, cur_to):
             self.crop_idx[self.inds[i]] += 1
+        # data parallel: the crop_idx of every chip of the global batch has moved on; this rank builds only its slice
+        mine = slice(self.chip_base, self.chip_base + self.slice_size)
+        entries, cropids = entries[mine], cropids[mine]
         # source rectangles (im_worker.worker: flip, then im[int(y1):int(y2), int(x1):int(x2)])
         rects = []
         for r, cid in zip(entries, cropids):
@@ -302,6 +362,8 @@ class MNIteratorE2E(object):
                     raw.focus_boxes[k, :len(fb)] = torch.from_numpy(np.ascontiguousarray(fb, dtype=np.float32))
         raw.used_pixels = off
         raw.seed = (self.epiter * 1000003 + self.cur_i) & 0x7FFFFFFF
+        raw.chip_base = self.chip_base
+        raw.plan_digest = self.plan_digest
         return raw
 
 
@@ -419,9 +481,10 @@ class InputStage(object):
                                           scales=self.scales, ratios=self.ratios, pos_thresh=self.pos,
                                           neg_thresh=self.neg)
         if subsample:
+            # keyed by the chip's position in the global batch: a data-parallel rank draws what the whole batch would
             A = len(self.scales) * len(self.ratios)
-            check(lib().sniper_anchor_subsample(label.data_ptr(), bt.data_ptr(), bw.data_ptr(), self.B, A, Hf, Hf,
-                                                self.num_fg, self.rpn_batch, int(raw.seed), st))
+            check(lib().sniper_anchor_subsample_at(label.data_ptr(), bt.data_ptr(), bw.data_ptr(), self.B, A, Hf, Hf,
+                                                   self.num_fg, self.rpn_batch, int(raw.seed), int(raw.chip_base), st))
         out = dict(data=self.data, label=label, bbox_target=bt, bbox_weight=bw, gt_boxes=self.dev["gt_boxes"],
                    valid_ranges=self.dev["valid_ranges"], im_info=self.dev["im_info"])
         if self.autofocus:

@@ -16,12 +16,32 @@ import logging
 import time
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import checkpoint, lr_scheduler, metric, model, ops
 
 # mxnet.model.BatchEndParam (SNIPER-mxnet/python/mxnet/model.py:51-56)
 BatchEndParam = namedtuple("BatchEndParams", ["epoch", "nbatch", "eval_metric", "locals"])
+
+
+def check_plan(digest, world_size, epoch=None):
+    """Collective: every rank passes the plan digest of its epoch's first raw batch (`RawBatch.plan_digest`, None when
+    the iterator gives none).  Raises ValueError on every rank, naming the ranks, when the ranks' plans differ, so
+    that no rank goes on into a collective the others never reach.  Digests that are None on every rank are not
+    checked."""
+    if world_size <= 1:
+        return
+    got = [None] * world_size
+    torch.distributed.all_gather_object(got, None if digest is None else int(digest))
+    if all(d is None for d in got) or all(d == got[0] for d in got):
+        return
+    groups = {}
+    for r, d in enumerate(got):
+        groups.setdefault(d, []).append(r)
+    raise ValueError("%sthe ranks' epoch plans differ (different iterator seeds, roidbs or configs?): %s" % (
+        "" if epoch is None else "epoch %d: " % epoch,
+        "; ".join("ranks %s: %s" % (rs, "no digest" if d is None else "%016x" % d) for d, rs in groups.items())))
 
 
 class Trainer:
@@ -169,6 +189,32 @@ class Trainer:
             w.wait()                              # the current stream waits for the collective
         self._works = []
 
+    def export_reference(self):
+        """net.export_reference() as a checkpoint holds it.  With several ranks this is a collective: every auxiliary
+        state (the BatchNorm moving statistics, which each rank updates from its own chips) is averaged over the ranks as
+        DataParallelExecutorGroup.get_params does (module/executor_group.py:415-420): float32, summed in rank order
+        starting from rank 0's value, then divided by the number of ranks.  The weights are identical on every rank."""
+        arg, aux = self.net.export_reference()
+        if self.world_size <= 1 or not aux:
+            return arg, aux
+        names = sorted(aux)
+        flat = torch.from_numpy(np.concatenate([np.ascontiguousarray(aux[k], np.float32).ravel() for k in names]))
+        if torch.distributed.get_backend() == "nccl":
+            flat = flat.to(self.device)
+        got = [torch.empty_like(flat) for _ in range(self.world_size)]
+        torch.distributed.all_gather(got, flat)
+        got = [g.cpu().numpy() for g in got]
+        total = got[0].copy()
+        for g in got[1:]:
+            total += g
+        total /= np.float32(self.world_size)
+        off = 0
+        for k in names:
+            n = aux[k].size
+            aux[k] = total[off:off + n].reshape(aux[k].shape).copy()
+            off += n
+        return arg, aux
+
     def _snapshot(self):
         P = self.net.P
         bns = self.net.train_bns()
@@ -294,11 +340,12 @@ class Trainer:
         return self._losses(self.step_device(lr))
 
     # ---- checkpoints (Module.save_checkpoint / load_optimizer_states, module.py:160-180, 775-805)
-    def save_checkpoint(self, prefix, epoch, save_optimizer_states=False):
+    def save_checkpoint(self, prefix, epoch, save_optimizer_states=False, arg_params=None, aux_params=None):
         """`<prefix>-%04d.params` through checkpoint.save_checkpoint (with the `*_test` box-regression tensors), the
         bound Symbol's `<prefix>-symbol.json` when the net came from one, and `<prefix>-%04d.states` (momenta and the
-        update count) when asked."""
-        arg, aux = self.net.export_reference()
+        update count) when asked.  arg_params / aux_params: what `export_reference()` returned (fit passes them to its
+        epoch-end callbacks); without them it is called here, which with several ranks is a collective."""
+        arg, aux = (arg_params, aux_params) if arg_params is not None else self.export_reference()
         sym = getattr(self.net, "symbol", None)
         if sym is not None:
             sym.save("%s-symbol.json" % prefix)
@@ -324,10 +371,16 @@ class Trainer:
 
         The host runs at most one step ahead of the device: before step i+1 is enqueued (and before its raw batch is
         taken from the iterator) step i-1 has completed, so at most two raw batches are read by in-flight H2D copies.
-        With several ranks every rank must call fit; metric reads are collective, and only rank 0 logs.  Every rank's
-        iterator must yield the same number of batches per epoch (the negative-chip draw sets it, so seed the ranks'
-        draws alike): a rank whose epoch ends early leaves the others waiting in a collective.  Not run on more than
-        one GPU yet."""
+        With several ranks every rank must call fit with its own `MNIteratorE2E(batch_size=W*B, nGPUs=W, rank=r,
+        seed=s)`, the same seed on every rank: each rank then takes its slice of every global batch, and all ranks
+        have the same epoch length.  At the first batch of every epoch fit all-gathers the batch's plan digest (on
+        this thread, so the collectives keep one order on every rank) and raises ValueError on every rank if they
+        differ.  Metric reads are collective, and only rank 0 logs.  The arg / aux params passed to
+        epoch_end_callback come from `export_reference()` (on every rank): the BatchNorm moving statistics averaged
+        over the ranks, as the reference's checkpoint holds them.  Verified with two ranks sharing one GPU over gloo
+        (tests/test_train_ranks_gpu.py, TF32 and bf16): after every epoch the weights and momenta are identical on both
+        ranks and byte-equal to a one-process emulation of the two slices with the gradients summed, and a resumed run
+        ends byte-equal to an uninterrupted one.  The test's NCCL variant needs two GPUs."""
         from . import iterator
         if isinstance(train_iter, iterator.PrefetchingIter) and not train_iter.epoch_marker:
             raise ValueError("fit: a PrefetchingIter needs epoch_marker=True (it would run one endless epoch)")
@@ -360,6 +413,7 @@ class Trainer:
             it = iter(train_iter)
             done = [None, None]                  # completion events of the last two steps enqueued
             next_raw = fetch(it)
+            check_plan(getattr(next_raw, "plan_digest", None), self.world_size, epoch)
             eval_name_vals = []
             while next_raw is not None:
                 raw = next_raw
@@ -380,7 +434,7 @@ class Trainer:
                     log.info("Epoch[%d] Train-%s=%f", epoch, name, val)
                 log.info("Epoch[%d] Time cost=%.3f", epoch, time.time() - tic)
             if epoch_end_callback is not None:
-                arg, aux = self.net.export_reference()
+                arg, aux = self.export_reference()
                 for cb in as_list(epoch_end_callback):
                     cb(epoch, getattr(self.net, "symbol", None), arg, aux)
             if not isinstance(train_iter, iterator.PrefetchingIter):

@@ -66,6 +66,7 @@ DOC = {
     "sniper_chip_input": "GPU input stage: im_worker.worker (lib/data_utils/data_workers.py:80-121) -- flip, cv2-style 8-bit bilinear resize by the chip scale, zero padding to crop_size, BGR->RGB minus PIXEL_MEANS -- from uint8 source rectangles to the fp32 NCHW `data` tensor of MNIteratorE2E (lib/iterators/MNIteratorE2E.py:194-199).",
     "sniper_chip_input_hw": "The same with a rectangular canvas: im_worker.worker_autofocus (lib/data_utils/data_workers.py:51-78) + the batch padding of MNIteratorTestAutoFocus._get_batch (lib/iterators/MNIteratorTestAutoFocus.py:36-78).",
     "sniper_anchor_subsample": "The npr.choice subsampling of anchor_worker.worker (data_workers.py:326-338) on device: <= num_fg positives, <= batch_size - #positives negatives per chip, the rest -> -1 (counter-based hash instead of numpy's RNG).",
+    "sniper_anchor_subsample_at": "sniper_anchor_subsample for chips [chip_base, chip_base + B) of a larger batch (data_workers.py:326-338): chip b draws what chip chip_base + b of one launch over the whole batch draws, so each data-parallel rank subsamples its slice of the global batch (MNIteratorE2E with rank=) as the whole batch would; chip_base = 0 is sniper_anchor_subsample.",
     "sniper_chips_generate": "chips::cgenerate (lib/chips/cchips.cpp:54-177): host-side chip sampling, same rand() stream.",
     "sniper_cpu_nms": "cpu_nms (lib/nms/cpu_nms.pyx:112-163), host.",
     "sniper_cpu_soft_nms": "cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110), host, in place.",

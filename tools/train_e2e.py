@@ -12,12 +12,26 @@ GT boxes only.  Images are read from disk by host.imread.  The network starts fr
 (checkpoint.load_param, then load_reference(allow_missing=True) as init_weight_rcnn: the layers an ImageNet checkpoint
 lacks keep their initialisation), otherwise from the constructor's initialisation.  The time of every roidb stage and of
 host.imread per image is logged and returned.
+
+Several GPUs, one process each (the reference trains on every GPU of config.gpus with one iterator of
+nGPUs * BATCH_IMAGES chips, main_train.py:44-45, 74):
+
+    python -m torch.distributed.run --nproc-per-node 8 tools/train_e2e.py --batch-size 20 --seed 0 ...
+
+Under torch.distributed.run (WORLD_SIZE > 1) the script joins an already initialised process group or initialises
+NCCL on cuda:LOCAL_RANK.  --batch-size stays per GPU; every rank runs MNIteratorE2E over the global batch of
+W * batch-size chips with its own rank and the same --seed and trains on its slice, Trainer sums the gradients.  Rank 0
+builds the roidb first (it writes the imdb caches), the other ranks then read them, and the ranks' roidbs are compared.
+Only rank 0 logs and writes checkpoints, and with --test-image-set rank 0 alone evaluates.  --begin-epoch N resumes
+from `<prefix>-N.params` / `.states` on every rank.
 """
 import argparse
 import logging
 import os
 import sys
 import time
+
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -44,8 +58,38 @@ def parse_args(argv=None):
     ap.add_argument("--prefix", default="output/SNIPER", help="checkpoint prefix (<prefix>-%%04d.params / .states)")
     ap.add_argument("--display", type=int, default=100, help="Speedometer period in batches")
     ap.add_argument("--test-image-set", default=None, help="after training, evaluate the last checkpoint on this set")
-    ap.add_argument("--device", default="cuda:0")
+    ap.add_argument("--device", default="cuda:0", help="the GPU (under torch.distributed.run with NCCL: cuda:LOCAL_RANK)")
+    ap.add_argument("--seed", type=int, default=None,
+                    help="seed of the iterator's draws, the same on every rank (default: the global np.random with one "
+                         "process, 0 with several)")
+    ap.add_argument("--begin-epoch", type=int, default=0,
+                    help="resume: load <prefix>-<N>.params / .states and train epochs N+1 .. --epochs")
     return ap.parse_args(argv)
+
+
+def init_distributed(args):
+    """-> (world size, rank).  Joins an initialised process group; otherwise, under a launcher with WORLD_SIZE > 1,
+    initialises NCCL on cuda:LOCAL_RANK (args.device is set to it).  One process: (1, 0), nothing initialised."""
+    dist = torch.distributed
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_world_size(), dist.get_rank()
+    if int(os.environ.get("WORLD_SIZE", "1")) <= 1:
+        return 1, 0
+    local = int(os.environ.get("LOCAL_RANK", "0"))
+    args.device = "cuda:%d" % local
+    torch.cuda.set_device(local)
+    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    return dist.get_world_size(), dist.get_rank()
+
+
+def _same_on_all_ranks(value, what, world):
+    """Collective: raises ValueError on every rank unless `value` is equal on all of them."""
+    if world <= 1:
+        return
+    got = [None] * world
+    torch.distributed.all_gather_object(got, value)
+    if any(v != got[0] for v in got):
+        raise ValueError("the ranks' %s differ: %s" % (what, ", ".join("rank %d: %r" % (r, v) for r, v in enumerate(got))))
 
 
 def config_for(args):
@@ -114,27 +158,44 @@ def imread_time(roidb, n=20):
     return (time.time() - t0) / max(len(paths), 1)
 
 
-def train(args, cfg, roidb, batch_end_callback=None, log=logging.getLogger()):
+def make_iterator(args, cfg, roidb, world=1, rank=0):
+    """MNIteratorE2E over the global batch of world * args.batch_size chips; with several ranks, this rank's slice of
+    it.  A resumed run (--begin-epoch N) skips the plans of the N epochs already trained."""
+    seed = args.seed if args.seed is not None or world == 1 else 0
+    it = IT.MNIteratorE2E(roidb, cfg, batch_size=world * args.batch_size, nGPUs=world, image_loader=host.imread,
+                          n_buffers=5, rank=None if world == 1 else rank, seed=seed)
+    for _ in range(args.begin_epoch):
+        it.reset()
+    return it
+
+
+def train(args, cfg, roidb, batch_end_callback=None, log=logging.getLogger(), world=1, rank=0):
     """The iterator over the roidb (images through host.imread) behind a PrefetchingIter, and Trainer.fit for
     args.epochs epochs with module_checkpoint and batch_end_callback (default: a Speedometer every args.display
-    batches).  Returns the trainer."""
+    batches, counting the chips of all ranks).  Returns the trainer."""
     os.makedirs(os.path.dirname(os.path.abspath(args.prefix)), exist_ok=True)
     B = args.batch_size
-    it = IT.MNIteratorE2E(roidb, cfg, batch_size=B, image_loader=host.imread, n_buffers=5)
+    it = make_iterator(args, cfg, roidb, world, rank)
     log.info("the iterator has %d chips", len(it))
     net = make_net(args, cfg.dataset.NUM_CLASSES, B, args.device)
-    if args.pretrained:
+    if args.begin_epoch > 0:
+        arg, aux = checkpoint.load_param(args.prefix, args.begin_epoch)
+        net.load_reference(arg, aux)
+        log.info("resuming from %s-%04d.params", args.prefix, args.begin_epoch)
+    elif args.pretrained:
         load_weights(net, args, args.pretrained, args.pretrained_epoch, log)
     net.cfg.roidb_len = len(it)            # the epoch boundaries of lr_step, as get_optim_params reads them
     if args.lr is not None:
         net.cfg.lr = args.lr
-    tr = trainer.Trainer(net.cfg, device=args.device, net=net)
+    tr = trainer.Trainer(net.cfg, device=args.device, net=net, world_size=world)
+    if args.begin_epoch > 0:
+        tr.load_optimizer_states("%s-%04d.states" % (args.prefix, args.begin_epoch))
     stage = IT.InputStage(cfg, args.device, B)
-    pf = IT.PrefetchingIter(it, depth=2, epochs=args.epochs, epoch_marker=True)
+    pf = IT.PrefetchingIter(it, depth=2, epochs=args.epochs - args.begin_epoch, epoch_marker=True)
     try:
         if batch_end_callback is None:
-            batch_end_callback = callback.Speedometer(B, args.display)
-        tr.fit(pf, stage, args.epochs, batch_end_callback=batch_end_callback,
+            batch_end_callback = callback.Speedometer(world * B, args.display)
+        tr.fit(pf, stage, args.epochs, begin_epoch=args.begin_epoch, batch_end_callback=batch_end_callback,
                epoch_end_callback=callback.module_checkpoint(tr, args.prefix))
     finally:
         pf.close()
@@ -167,20 +228,37 @@ def evaluate(args, cfg, epoch, log=logging.getLogger()):
 
 
 def main(argv=None, batch_end_callback=None):
-    """Roidb, training and (with --test-image-set) evaluation.  Returns dict(times, bbox_means, bbox_stds, trainer,
-    and all_boxes / stats of the evaluation)."""
-    logging.basicConfig(level=logging.INFO, format="%(asctime)s %(message)s")
-    log = logging.getLogger()
+    """Roidb, training and (with --test-image-set) evaluation on rank 0.  Returns dict(times, bbox_means, bbox_stds,
+    trainer, world_size, rank, and all_boxes / stats of the evaluation).  A process group this call initialised is
+    destroyed before it returns."""
     args = parse_args(argv)
-    cfg = config_for(args)
-    roidb, bbox_means, bbox_stds, times = build_roidb(args, cfg, log)
-    times["imread_s_per_image"] = imread_time(roidb)
-    log.info("host.imread: %.4f s per image", times["imread_s_per_image"])
-    tr = train(args, cfg, roidb, batch_end_callback, log)
-    out = dict(times=times, bbox_means=bbox_means, bbox_stds=bbox_stds, trainer=tr)
-    if args.test_image_set:
-        out["all_boxes"], out["stats"] = evaluate(args, cfg, args.epochs, log)
-    return out
+    dist = torch.distributed
+    owned = not (dist.is_available() and dist.is_initialized())
+    world, rank = init_distributed(args)
+    logging.basicConfig(level=logging.INFO if rank == 0 else logging.WARNING, format="%(asctime)s %(message)s")
+    log = logging.getLogger()
+    try:
+        cfg = config_for(args)
+        # rank 0 first: it writes the imdb caches and the proposals' _rpn_after_nms.pkl the other ranks then read
+        if rank == 0:
+            roidb, bbox_means, bbox_stds, times = build_roidb(args, cfg, log)
+        if world > 1:
+            dist.barrier()
+            if rank != 0:
+                roidb, bbox_means, bbox_stds, times = build_roidb(args, cfg, log)
+            _same_on_all_ranks(IT.roidb_digest(roidb), "training roidbs", world)
+        times["imread_s_per_image"] = imread_time(roidb)
+        log.info("host.imread: %.4f s per image", times["imread_s_per_image"])
+        tr = train(args, cfg, roidb, batch_end_callback, log, world, rank)
+        out = dict(times=times, bbox_means=bbox_means, bbox_stds=bbox_stds, trainer=tr, world_size=world, rank=rank)
+        if world > 1:
+            dist.barrier()                 # rank 0 has written the last checkpoint
+        if args.test_image_set and rank == 0:
+            out["all_boxes"], out["stats"] = evaluate(args, cfg, args.epochs, log)
+        return out
+    finally:
+        if owned and world > 1:
+            dist.destroy_process_group()
 
 
 if __name__ == "__main__":
