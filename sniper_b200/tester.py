@@ -1,9 +1,10 @@
 """AutoFocus multi-scale inference: the test iterator, `Tester` and the scale pyramid driver.
 
 Host-side mirror of `lib/iterators/MNIteratorTestAutoFocus.py` (:13-141), `lib/inference.py` `Tester.detect` (:100-139),
-`Tester.get_detections` (:232-370), `Tester.aggregate` (:152-230, in `inference.aggregate`) and the single-job branch of
-`imdb_detection_wrapper` / `detect_scale_worker` (:400-528): same names, argument meaning and returned structures
-(`all_boxes[class][image][chip]`, `all_maps[image][chip]`).  What changes is where the arithmetic runs:
+`Tester.get_detections` (:232-370), `Tester.aggregate` (:152-230, in `inference.aggregate`) and
+`imdb_detection_wrapper` / `detect_scale_worker` (:400-528), TEST.CONCURRENT_JOBS included: same names, argument
+meaning and returned structures (`all_boxes[class][image][chip]`, `all_maps[image][chip]`).  What changes is where the
+arithmetic runs:
 
   reference                                             here
   cv2 crop / resize / pad in a thread pool              one `sniper_chip_input_hw` launch per batch (uint8 crops over PCIe)
@@ -392,24 +393,91 @@ class Tester(object):
                                    device=str(self.net.device) if self.net is not None else "cuda")
 
 
-def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device",
-                           imdb=None, detect_backend="host", image_loader=None):
-    """The CONCURRENT_JOBS == 1 path of imdb_detection_wrapper (:436-528): every scale of TEST.SCALES in turn (FocusChips
-    of scale i feed scale i + 1 when DO_PRUNING[i + 1]), then the cross-scale aggregation.
-    Returns (all_boxes[class][image], stats) with per-scale chip counts / detect / post-processing seconds, the NMS
-    latency and the pixel fraction processed.  detect_backend="device" keeps the detections on the GPU from the network
-    to the soft-NMS (`Tester.get_detections(backend="device")`); stats then carry `detections_pre_nms` per scale.
-    With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
-    dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
-    and its seconds to stats['eval_s'].  `net` is a `DetectionNetwork`; config is the network's own (e.g.
-    iterator.default_config(network="mobilenetv2") for a SniperMobileNetV2): its RPN_FEAT_STRIDE must be the net's.
-    image_loader(path) decodes the entries without 'image_data' (e.g. host.imread)."""
+def job_blocks(num_images, jobs):
+    """The image range [lo, hi) of each of `jobs` concurrent test jobs, in job order, as the reference's wrappers split
+    the roidb for TEST.CONCURRENT_JOBS > 1 (:457-461, 568-572): im_per_job = ceil(N / jobs) images per job, so the
+    trailing blocks can be short or empty (N = 5, jobs = 4: 2, 2, 1 and 0 images)."""
+    if int(jobs) != jobs or jobs < 1:
+        raise ValueError("concurrent_jobs must be a positive integer, not %r" % (jobs,))
+    per = -(-num_images // jobs)
+    return [(min(per * j, num_images), min(per * (j + 1), num_images)) for j in range(jobs)]
+
+
+def _world(group):
+    if group is None:
+        return 1, 0
+    return torch.distributed.get_world_size(group), torch.distributed.get_rank(group)
+
+
+def _same_on_all_ranks(value, what, group):
+    """Collective: raises ValueError on every rank of `group` unless `value` is equal on all of them."""
+    got = [None] * _world(group)[0]
+    torch.distributed.all_gather_object(got, value, group=group)
+    if any(v != got[0] for v in got):
+        raise ValueError("the ranks' %s differ: %s" % (what, ", ".join("rank %d: %r" % (r, v) for r, v in enumerate(got))))
+
+
+def _test_roidb_digest(roidb):
+    """iterator.roidb_digest of a test roidb, whose entries may carry no GT boxes."""
+    from .iterator import roidb_digest
+    return roidb_digest([r if 'boxes' in r else dict(r, boxes=np.zeros((0, 4))) for r in roidb])
+
+
+def _concurrent_jobs(roidb, jobs, group, run_job):
+    """Runs run_job(block) -> (result, stats) on the roidb block of every job (`job_blocks`) and yields (result, job
+    stats) in job order.  A job's stats are dict(images=(lo, hi), rank=<rank it ran on>) plus run_job's own; an empty
+    block runs nothing and yields (None, dict(images, rank, scales=[])).
+
+    With a process group of W ranks, job j runs on rank j mod W, W jobs at a time.  Each job's result then goes to
+    rank 0 on its own (point to point, in job order), so rank 0 holds at most one received result beyond what its
+    caller has merged, and nothing is all-gathered.  Rank 0 yields every job; another rank yields (None, stats) for its
+    own jobs only.  Before any work the ranks compare the roidb's digest and `jobs`; before each round's results move
+    they share every job's success or failure, so an exception on one rank (a detect_post capacity error, say) raises
+    RuntimeError with that rank's message on every rank instead of leaving the others waiting in a collective."""
+    world, rank = _world(group)
+    if world > 1:
+        _same_on_all_ranks((_test_roidb_digest(roidb), int(jobs)), "test roidbs and concurrent_jobs", group)
+    blocks = job_blocks(len(roidb), jobs)
+    dist = torch.distributed
+    for first in range(0, jobs, world):
+        j = first + rank
+        result = st = err = failure = None
+        if j < jobs:
+            lo, hi = blocks[j]
+            st = dict(images=(lo, hi), rank=rank, scales=[])
+            if hi > lo:
+                try:
+                    result, job_st = run_job(roidb[lo:hi])
+                    st.update(job_st)
+                except Exception as e:
+                    if world == 1:
+                        raise
+                    err, failure = "%s: %s" % (type(e).__name__, e), e
+        if world > 1:
+            errs = [None] * world
+            dist.all_gather_object(errs, err, group=group)
+            bad = [(r, e) for r, e in enumerate(errs) if e is not None]
+            if bad:
+                raise RuntimeError("; ".join("concurrent test job %d (images %d:%d) failed on rank %d: %s"
+                                             % ((first + r,) + tuple(blocks[first + r]) + (r, e)) for r, e in bad)
+                                   ) from failure
+        for k in range(first, min(first + world, jobs)):
+            owner = k - first
+            if owner == rank:
+                if rank != 0:
+                    dist.send_object_list([result, st], group=group, group_dst=0)
+                    result = None
+                yield result, st
+            elif rank == 0:
+                got = [None, None]
+                dist.recv_object_list(got, group=group, group_src=owner)
+                yield got[0], got[1]
+
+
+def _detection_job(net, config, roidb, num_classes, batch_images, device, nms_backend, detect_backend, image_loader):
+    """One test job: every scale of TEST.SCALES over `roidb` in turn (FocusChips of scale i feed scale i + 1 when
+    DO_PRUNING[i + 1]), then the cross-scale aggregation.  Returns (all_boxes[class][image], stats)."""
     T = config.TEST
-    if int(config.network.RPN_FEAT_STRIDE) != int(net.feat_stride):
-        raise ValueError("imdb_detection_wrapper: config.network.RPN_FEAT_STRIDE is %s, the network's stride is %s"
-                         % (config.network.RPN_FEAT_STRIDE, net.feat_stride))
-    for r in roidb:
-        r['inference_crops'] = np.array([[0, 0, r['width'], r['height']]])
     detections, stats = [], dict(scales=[])
     nb = batch_images or list(T.BATCH_IMAGES)
     for scale_i, (nbatch, scale) in enumerate(zip(nb, T.SCALES)):
@@ -434,6 +502,56 @@ def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=No
     all_boxes = tester.aggregate(detections, backend=nms_backend)
     torch.cuda.synchronize()
     stats['nms_s'] = time.time() - t0
+    return all_boxes, stats
+
+
+def imdb_detection_wrapper(net, config, roidb, num_classes=None, batch_images=None, device="cuda:0", nms_backend="device",
+                           imdb=None, detect_backend="host", image_loader=None, concurrent_jobs=1, group=None):
+    """imdb_detection_wrapper (:436-528): every scale of TEST.SCALES in turn (FocusChips of scale i feed scale i + 1 when
+    DO_PRUNING[i + 1]), then the cross-scale aggregation.
+    Returns (all_boxes[class][image], stats) with per-scale chip counts / detect / post-processing seconds, the NMS
+    latency and the pixel fraction processed.  detect_backend="device" keeps the detections on the GPU from the network
+    to the soft-NMS (`Tester.get_detections(backend="device")`); stats then carry `detections_pre_nms` per scale.
+    With an imdb (e.g. `coco.coco`, whose gt_roidb is `roidb`), the
+    dataset evaluation of :526-527 follows: imdb.evaluate_detections(all_boxes), whose result goes to stats['eval']
+    and its seconds to stats['eval_s'].  `net` is a `DetectionNetwork`; config is the network's own (e.g.
+    iterator.default_config(network="mobilenetv2") for a SniperMobileNetV2): its RPN_FEAT_STRIDE must be the net's.
+    image_loader(path) decodes the entries without 'image_data' (e.g. host.imread).
+
+    concurrent_jobs=J > 1 is TEST.CONCURRENT_JOBS: the images are split into J blocks (`job_blocks`) and each block runs
+    the whole pipeline above on its own -- its own test iterators (so chips are sorted, grouped and padded per block),
+    its own add_chips and its own aggregation -- and all_boxes[j] is the jobs' lists concatenated per class in job
+    order.  That is the reference's result, where the jobs' per-scale outputs are merged and then aggregated once:
+    the soft-NMS solves one (image, class) problem at a time, the MAX_PER_IMAGE cut is per image and add_chips works
+    per image, so no image's result depends on which block it is in.  (With the device backend a job's run keys carry
+    block-local image indices; each job aggregates its own rows, no run buffer spans two jobs.)
+    group=<process group of W ranks> runs job j on rank j mod W (`_concurrent_jobs`), each rank on its own `net` /
+    `device`, reading only its jobs' images.  Rank 0 merges and evaluates; the other ranks return (None, stats).  The
+    group is never taken from torch.distributed implicitly: a caller that evaluates on one rank of a larger group passes
+    none.  With J > 1 or a group, stats holds `jobs` (per job: images (lo, hi), rank, and the per-scale `scales` and
+    `nms_s` of that job) instead of `scales` / `nms_s`; `eval` / `eval_s` stay as above, on rank 0."""
+    if int(config.network.RPN_FEAT_STRIDE) != int(net.feat_stride):
+        raise ValueError("imdb_detection_wrapper: config.network.RPN_FEAT_STRIDE is %s, the network's stride is %s"
+                         % (config.network.RPN_FEAT_STRIDE, net.feat_stride))
+    job_blocks(len(roidb), concurrent_jobs)
+    for r in roidb:
+        r['inference_crops'] = np.array([[0, 0, r['width'], r['height']]])
+
+    def run_job(block):
+        return _detection_job(net, config, block, num_classes, batch_images, device, nms_backend, detect_backend,
+                              image_loader)
+    if concurrent_jobs == 1 and group is None:
+        all_boxes, stats = run_job(roidb)
+    else:
+        all_boxes = [[] for _ in range(num_classes or config.dataset.NUM_CLASSES)]
+        stats = dict(jobs=[])
+        for boxes, st in _concurrent_jobs(roidb, concurrent_jobs, group, run_job):
+            stats['jobs'].append(st)
+            if boxes is not None:
+                for c, per_image in zip(all_boxes, boxes):
+                    c += per_image
+        if _world(group)[1] != 0:
+            return None, stats
     if imdb is not None:
         t0 = time.time()
         stats['eval'] = imdb.evaluate_detections(all_boxes)
@@ -446,16 +564,9 @@ def proposal_file_name(config):
     return '{}_{}_rpn.pkl'.format(config.dataset.dataset.upper(), config.dataset.test_image_set)
 
 
-def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0",
-                                     image_loader=None, imdb=None):
-    """The CONCURRENT_JOBS == 1 path of imdb_proposal_extraction_wrapper (:559-610): RPN proposals of every image at every
-    scale of TEST.SCALES (`net.forward_rpn`), each image's rows stacked in scale order, pickled as a list of float32
-    [n, 5] arrays to save_path/proposal_file_name(config) (protocol 2, readable by the reference's Python 2).  Returns
-    (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds.  image_loader(path)
-    decodes the entries without 'image_data' (e.g. host.imread).  With an imdb (`coco.coco`, `pascal_voc.PascalVOC`
-    or `proposals.IMDB`), the recall of the extracted proposals follows: imdb.evaluate_recall(roidb, candidate_boxes=
-    [p[:, :4] for p in proposals]) against the GT fields of `roidb` (boxes / gt_classes / gt_overlaps), whose string
-    goes to stats['recall'] and its seconds to stats['recall_s']."""
+def _proposal_job(net, config, roidb, batch_images, n_proposals, device, image_loader):
+    """One extraction job: RPN proposals of every image of `roidb` at every scale of TEST.SCALES, each image's rows
+    stacked in scale order.  Returns (proposals[image], stats)."""
     T = config.TEST
     proposals, stats = [], dict(scales=[])
     nb = batch_images or list(T.BATCH_IMAGES)
@@ -466,7 +577,40 @@ def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images
         proposals.append(tester.extract_proposals(n_proposals=n_proposals))
         stats['scales'].append(dict(scale=tuple(scale), images=len(roidb), batches=int(it.size // max(nbatch, 1)),
                                     detect_s=tester.detect_time, post_s=tester.post_time, total_s=time.time() - t0))
-    final = [np.vstack([p[i] for p in proposals]) for i in range(len(roidb))]
+    return [np.vstack([p[i] for p in proposals]) for i in range(len(roidb))], stats
+
+
+def imdb_proposal_extraction_wrapper(net, config, roidb, save_path, batch_images=None, n_proposals=300, device="cuda:0",
+                                     image_loader=None, imdb=None, concurrent_jobs=1, group=None):
+    """imdb_proposal_extraction_wrapper (:559-610): RPN proposals of every image at every scale of TEST.SCALES
+    (`net.forward_rpn`), each image's rows stacked in scale order, pickled as a list of float32 [n, 5] arrays to
+    save_path/proposal_file_name(config) (protocol 2, readable by the reference's Python 2).  Returns
+    (proposals, stats) with per-scale image / batch counts and forward / post-processing seconds.  image_loader(path)
+    decodes the entries without 'image_data' (e.g. host.imread).  With an imdb (`coco.coco`, `pascal_voc.PascalVOC`
+    or `proposals.IMDB`), the recall of the extracted proposals follows: imdb.evaluate_recall(roidb, candidate_boxes=
+    [p[:, :4] for p in proposals]) against the GT fields of `roidb` (boxes / gt_classes / gt_overlaps), whose string
+    goes to stats['recall'] and its seconds to stats['recall_s'].
+
+    concurrent_jobs / group split the images into jobs and run them on the ranks as `imdb_detection_wrapper` does; the
+    jobs' lists are concatenated in job order, which is the reference's result: it stacks each image's rows per image.
+    Rank 0 writes the pickle and scores the recall; the other ranks write nothing and return (None, stats).  With
+    J > 1 or a group, stats holds `jobs` (per job: images (lo, hi), rank and its `scales`) instead of `scales`."""
+    job_blocks(len(roidb), concurrent_jobs)
+
+    def run_job(block):
+        return _proposal_job(net, config, block, batch_images, n_proposals, device, image_loader)
+    if concurrent_jobs == 1 and group is None:
+        final, stats = run_job(roidb)
+    else:
+        final, stats = [], dict(jobs=[])
+        for props, st in _concurrent_jobs(roidb, concurrent_jobs, group, run_job):
+            stats['jobs'].append(st)
+            if props is not None:
+                # an array received from another rank carries an unpickled float32 dtype object, equal to but not the
+                # one of local arrays, which pickle would write once more: the file must not depend on the ranks
+                final += [np.asarray(p, np.float32) for p in props]
+        if _world(group)[1] != 0:
+            return None, stats
     os.makedirs(save_path, exist_ok=True)
     with open(os.path.join(save_path, proposal_file_name(config)), 'wb') as f:
         pickle.dump(final, f, protocol=2)

@@ -202,13 +202,10 @@ def train(args, cfg, roidb, batch_end_callback=None, log=logging.getLogger(), wo
     return tr
 
 
-def evaluate(args, cfg, epoch, log=logging.getLogger()):
-    """tester.imdb_detection_wrapper on args.test_image_set with `<prefix>-<epoch>.params` (the `*_test` box-regression
-    tensors, as main_test.py loads them) and the imdb's evaluation.  Returns (all_boxes, stats)."""
-    from sniper_b200 import tester
-    imdb = load_data.DATASETS[args.dataset](args.test_image_set, args.root_path, args.dataset_path,
-                                            os.path.dirname(os.path.abspath(args.prefix)), device=args.device)
-    db = [dict(image=r['image'], width=int(r['width']), height=int(r['height'])) for r in imdb.gt_roidb()]
+def load_test_net(args, cfg, epoch):
+    """The network of `<prefix>-<epoch>.params` for inference, with the `*_test` box-regression tensors as main_test.py
+    loads them (checkpoint.load_param(process=True)).  For a network without the FocusPixel branch, cfg.TEST's
+    AUTO_FOCUS / DO_PRUNING are turned off: plain multi-scale inference."""
     net = make_net(args, cfg.dataset.NUM_CLASSES, 1, args.device)
     arg, aux = checkpoint.load_param(args.prefix, epoch, process=True)
     if args.network == "mobilenetv2":
@@ -218,8 +215,18 @@ def evaluate(args, cfg, epoch, log=logging.getLogger()):
     if args.network == "resnet101_autofocus":
         net.enable_autofocus(arg=arg)
     elif cfg.TEST.AUTO_FOCUS:
-        # a network trained without the FocusPixel branch: plain multi-scale inference
         cfg.TEST.AUTO_FOCUS, cfg.TEST.DO_PRUNING = False, [False] * len(cfg.TEST.SCALES)
+    return net
+
+
+def evaluate(args, cfg, epoch, log=logging.getLogger()):
+    """tester.imdb_detection_wrapper on args.test_image_set with `<prefix>-<epoch>.params` (the `*_test` box-regression
+    tensors, as main_test.py loads them) and the imdb's evaluation.  Returns (all_boxes, stats)."""
+    from sniper_b200 import tester
+    imdb = load_data.DATASETS[args.dataset](args.test_image_set, args.root_path, args.dataset_path,
+                                            os.path.dirname(os.path.abspath(args.prefix)), device=args.device)
+    db = [dict(image=r['image'], width=int(r['width']), height=int(r['height'])) for r in imdb.gt_roidb()]
+    net = load_test_net(args, cfg, epoch)
     all_boxes, stats = tester.imdb_detection_wrapper(net, cfg, db, num_classes=cfg.dataset.NUM_CLASSES,
                                                      device=args.device, imdb=imdb, detect_backend="device",
                                                      image_loader=host.imread)
