@@ -77,6 +77,11 @@ SIGNATURES = {
     "sniper_anchor_subsample": ("i", "pppiiiiiiup"),
     "sniper_anchor_subsample_at": ("i", "pppiiiiiiuip"),
     "sniper_chips_generate": ("i", "piiiiipi"),
+    "sniper_chips_shuffle": ("i", "pip"),
+    "sniper_chip_plan_layout": ("i", "piiip"),
+    "sniper_chip_plan_count": ("i", "ppiiii" "pppp" "p"),
+    "sniper_chip_plan_cover": ("i", "ppiiiii" "pppppp" "pl" "ppp" "p"),
+    "sniper_chip_plan_assign": ("i", "ppiii" "pppppppp" "p"),
     "sniper_cpu_nms": ("i", "ppidp"),
     "sniper_cpu_soft_nms": ("i", "pifffu"),
     "sniper_bbox_overlaps": ("i", "pipipi"),
@@ -100,7 +105,7 @@ _lib = None
 KERNELS_PER_CALL = {
     "sniper_last_error": 0, "sniper_abi_version": 0, "sniper_stream_workspace_bytes": 0,
     "sniper_set_stream_workspace": 0, "sniper_multi_proposal_target_workspace_bytes": 0,
-    "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
+    "sniper_generate_anchors": 0, "sniper_chips_generate": 0, "sniper_chips_shuffle": 0, "sniper_chip_plan_layout": 0, "sniper_cpu_nms": 0, "sniper_cpu_soft_nms": 0,
     "sniper_bbox_overlaps": 0, "sniper_gemm_plan": 0, "sniper_detect_post_workspace_bytes": 0, "sniper_train_metric_workspace_bytes": 0,
     "sniper_proposal_recall_workspace_bytes": 0, "sniper_focus_chips_workspace_bytes": 0, "sniper_multi_proposal_target_fwd": 2, "sniper_multi_proposal_workspace_bytes": 0, "sniper_multi_proposal_fwd": 4, "sniper_anchor_target": 2, "sniper_bn_stats": 2, "sniper_bn_relu_bwd": 2, "sniper_bn_act_bwd": 2,
     "sniper_deform_col2im_fp64acc": 2, "sniper_deform_psroi_bwd_fp64acc": 2,

@@ -21,6 +21,16 @@ struct Box4 {
   float x1, y1, x2, y2;
 };
 
+// 0 .. n-1 in the order std::random_shuffle of libstdc++ (bits/stl_algo.h) leaves them: for i in 1..n-1:
+// swap(ids[i], ids[rand() % (i+1)]); n - 1 draws from rand()
+void shuffled_ids(int* ids, int n) {
+  std::iota(ids, ids + n, 0);
+  for (int i = 1; i < n; ++i) {
+    const int j = rand() % (i + 1);
+    if (i != j) std::swap(ids[i], ids[j]);
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -47,12 +57,7 @@ int sniper_chips_generate(const float* boxes, int num_boxes, int width, int heig
     push((float)i, (float)std::max(height - chipsize - 1, 0), (float)(i + chipsize - 1), (float)(height - 1));
   const int n = (int)cand.size();
   std::vector<int> ids(n);
-  std::iota(ids.begin(), ids.end(), 0);
-  // std::random_shuffle of libstdc++ (bits/stl_algo.h): for i in 1..n-1: swap(ids[i], ids[rand() % (i+1)])
-  for (int i = 1; i < n; ++i) {
-    const int j = rand() % (i + 1);
-    if (i != j) std::swap(ids[i], ids[j]);
-  }
+  shuffled_ids(ids.data(), n);
   const int words = (num_boxes + 63) / 64;
   std::vector<uint64_t> match((size_t)n * words, 0);
   std::vector<int> count(n, 0);
@@ -101,6 +106,26 @@ int sniper_chips_generate(const float* boxes, int num_boxes, int width, int heig
     }
   }
   return nout;
+}
+
+// The candidate orders of a sequence of sniper_chips_generate calls, drawn from rand() as those calls draw them: call c
+// has n_cand[c] candidates (0: a call without boxes, which draws nothing) and its order goes to
+// perm_out[sum(n_cand[:c]) ...].  rand() ends where it would after the calls.  Refuses before drawing anything.
+int sniper_chips_shuffle(const int* n_cand, int n_calls, int* perm_out) {
+  SN_CHECK(n_calls >= 0, "chips_shuffle: n_calls (%d) must not be negative", n_calls);
+  SN_CHECK(n_calls == 0 || n_cand, "chips_shuffle: n_cand must not be null");
+  long total = 0;
+  for (int c = 0; c < n_calls; ++c) {
+    SN_CHECK(n_cand[c] >= 0, "chips_shuffle: call %d has %d candidates", c, n_cand[c]);
+    total += n_cand[c];
+  }
+  SN_CHECK(total == 0 || perm_out, "chips_shuffle: perm_out must not be null");
+  long off = 0;
+  for (int c = 0; c < n_calls; ++c) {
+    shuffled_ids(perm_out + off, n_cand[c]);
+    off += n_cand[c];
+  }
+  return 0;
 }
 
 // dets: host float[n,5]; order: host int64[n] = scores.argsort()[::-1] (or NULL: stable descending order is

@@ -149,7 +149,7 @@ def roidb_digest(roidb):
 
 class MNIteratorE2E(object):
     def __init__(self, roidb, config, batch_size=4, threads=8, nGPUs=1, pad_rois_to=400, crop_size=(512, 512),
-                 image_loader=None, n_buffers=3, rank=None, seed=None):
+                 image_loader=None, n_buffers=3, rank=None, seed=None, plan_backend="host", device=None):
         """roidb entries: 'image' (path) or 'image_data' (decoded uint8 HxWx3 BGR), 'width', 'height', 'boxes' [n,4],
         'max_overlaps' (== 1 for GT rows), 'max_classes', 'flipped'.  image_loader(path) -> uint8 BGR array replaces
         cv2.imread (this image has no OpenCV).
@@ -161,7 +161,14 @@ class MNIteratorE2E(object):
         seed=int: every draw of an epoch comes from a private np.random.RandomState(seed) -- the chip stride, the
         negative-chip pick, the chip permutation, each image's chip_order -- and each epoch seeds the C rand() stream
         of the chip generator from it; seed=None draws from the global np.random (the reference's behaviour).  rank
-        needs a seed: the plan is computed on the prefetch thread, where the global state cannot be shared."""
+        needs a seed: the plan is computed on the prefetch thread, where the global state cannot be shared.
+        plan_backend="device" computes each epoch's chips, box assignment and negative chips (chip_worker's
+        chip_extractor / box_assigner) on `device` (default: the current CUDA device) with chip_plan.DevicePlan, on its
+        own stream; the result, including the rand() stream's position, is the host's.  The stride draw, the rand()
+        seeding, the negative-chip pick, the permutation and chip_order stay on the host.  The device plan reads the
+        roidb's boxes and sizes once, here."""
+        if plan_backend not in ("host", "device"):
+            raise ValueError("MNIteratorE2E: plan_backend must be 'host' or 'device', not %r" % (plan_backend,))
         assert batch_size % nGPUs == 0, 'batch_size should be divisible by number of GPUs'
         if rank is not None:
             if seed is None:
@@ -182,6 +189,11 @@ class MNIteratorE2E(object):
         self.image_loader = image_loader
         self.pixel_mean = config.network.PIXEL_MEANS
         self.chip_worker = chip_worker(chip_size=self.crop_size[0], cfg=config, rng=self.rng)
+        self.plan_backend = plan_backend
+        self._device_plan = None
+        if plan_backend == "device":
+            from .chip_plan import DevicePlan
+            self._device_plan = DevicePlan(roidb, self.chip_worker, device)
         self.max_gt = 100
         self.data_name = ['data', 'valid_ranges', 'im_info']
         self.label_name = ['label', 'bbox_target', 'bbox_weight', 'gt_boxes']
@@ -209,15 +221,19 @@ class MNIteratorE2E(object):
         if self.rng is not None:
             host.srand(int(self.rng.randint(0, 2 ** 31)))
         chip_count = 0
-        for r in self.roidb:
-            r['crops'] = self.chip_worker.chip_extractor(r)
-            chip_count += len(r['crops'])
-        for r in self.roidb:
-            ps = self.chip_worker.box_assigner(r)
-            r['props_in_chips'] = ps[0]
-            if self.cfg.TRAIN.USE_NEG_CHIPS:
-                r['neg_crops'] = ps[1]
-                r['neg_props_in_chips'] = ps[2]
+        if self._device_plan is not None:
+            self._device_plan.plan(self.roidb)
+            chip_count = sum(len(r['crops']) for r in self.roidb)
+        else:
+            for r in self.roidb:
+                r['crops'] = self.chip_worker.chip_extractor(r)
+                chip_count += len(r['crops'])
+            for r in self.roidb:
+                ps = self.chip_worker.box_assigner(r)
+                r['props_in_chips'] = ps[0]
+                if self.cfg.TRAIN.USE_NEG_CHIPS:
+                    r['neg_crops'] = ps[1]
+                    r['neg_props_in_chips'] = ps[2]
         chipindex = []
         for i, r in enumerate(self.roidb):
             if self.cfg.TRAIN.USE_NEG_CHIPS:

@@ -68,6 +68,11 @@ DOC = {
     "sniper_anchor_subsample": "The npr.choice subsampling of anchor_worker.worker (data_workers.py:326-338) on device: <= num_fg positives, <= batch_size - #positives negatives per chip, the rest -> -1 (counter-based hash instead of numpy's RNG).",
     "sniper_anchor_subsample_at": "sniper_anchor_subsample for chips [chip_base, chip_base + B) of a larger batch (data_workers.py:326-338): chip b draws what chip chip_base + b of one launch over the whole batch draws, so each data-parallel rank subsamples its slice of the global batch (MNIteratorE2E with rank=) as the whole batch would; chip_base = 0 is sniper_anchor_subsample.",
     "sniper_chips_generate": "chips::cgenerate (lib/chips/cchips.cpp:54-177): host-side chip sampling, same rand() stream.",
+    "sniper_chips_shuffle": "Host-only: the candidate orders of a sequence of sniper_chips_generate calls (std::random_shuffle over rand(), n_cand[c] - 1 draws per call; n_cand[c] = 0 is a call without boxes and draws nothing), written back to back to perm_out.  rand() ends where the calls would leave it.",
+    "sniper_chip_plan_layout": "Host-only: fills the workspace column of a chip-plan table (the byte offset of each cover whose scratch does not fit in shared memory, -1 for the others) and the workspace size sniper_chip_plan_cover then needs.  The library never allocates the workspace.",
+    "sniper_chip_plan_count": "The GT boxes chip_worker.chip_extractor (lib/data_utils/data_workers.py:394-450) selects for every (entry, scale) call of a chip-plan table in ONE launch: the integer size, fit and width / height tests of the host in float64.",
+    "sniper_chip_plan_cover": "chips::cgenerate (lib/chips/cchips.cpp:54-177) for every (entry, scale) call of a chip-plan table in ONE launch, one block per call: mode 0 over the GT boxes chip_extractor selects (data_workers.py:394-450), mode 1 over the boxes no positive chip kept (box_assigner's negative chips, :540-594).  Boxes scaled and clipped as chip_generator does, the candidate order read from perm (sniper_chips_shuffle), the float32 containment test, the first-maximum greedy cover.  Writes each call's chips in pick order as float32 and divided by the scale in float64, and their count.  Bit-exact (no FMA).",
+    "sniper_chip_plan_assign": "The box -> chip assignment of box_assigner (data_workers.py:452-594) for every call of a chip-plan table in ONE launch: owner = the first arg-max over the call's chips of the float64 ignore_overlaps (lib/bbox/bbox.pyx:59-95), kept iff the intersection is >= 1 on both sides and its sqrt-area in the scale's range (mode 0: positive chips, <= hi; mode 1: negative chips over the uncovered boxes, < hi).  owner_out int16 [boxes, S]: the owner, -1 selected but not kept, -2 not selected; left_count the selected boxes not kept.  Bit-exact (no FMA).",
     "sniper_cpu_nms": "cpu_nms (lib/nms/cpu_nms.pyx:112-163), host.",
     "sniper_cpu_soft_nms": "cpu_soft_nms (lib/nms/cpu_nms.pyx:17-110), host, in place.",
     "sniper_bbox_overlaps": "bbox_overlaps_cython / ignore_overlaps_cython (lib/bbox/bbox.pyx:17-95), host, float64.",

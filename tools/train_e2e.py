@@ -62,6 +62,9 @@ def parse_args(argv=None):
     ap.add_argument("--seed", type=int, default=None,
                     help="seed of the iterator's draws, the same on every rank (default: the global np.random with one "
                          "process, 0 with several)")
+    ap.add_argument("--plan-backend", default="host", choices=("host", "device"),
+                    help="where each epoch's chip plan (chips, box assignment, negative chips) is computed; the device "
+                         "plan is byte-equal to the host one")
     ap.add_argument("--begin-epoch", type=int, default=0,
                     help="resume: load <prefix>-<N>.params / .states and train epochs N+1 .. --epochs")
     return ap.parse_args(argv)
@@ -163,7 +166,9 @@ def make_iterator(args, cfg, roidb, world=1, rank=0):
     it.  A resumed run (--begin-epoch N) skips the plans of the N epochs already trained."""
     seed = args.seed if args.seed is not None or world == 1 else 0
     it = IT.MNIteratorE2E(roidb, cfg, batch_size=world * args.batch_size, nGPUs=world, image_loader=host.imread,
-                          n_buffers=5, rank=None if world == 1 else rank, seed=seed)
+                          n_buffers=5, rank=None if world == 1 else rank, seed=seed,
+                          plan_backend=getattr(args, "plan_backend", "host"),
+                          device=args.device if getattr(args, "plan_backend", "host") == "device" else None)
     for _ in range(args.begin_epoch):
         it.reset()
     return it
